@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- InternVLA-N1 policy-steps/sec on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py -- InternVLA-N1 policy-steps/sec on H100 (BASELINE.json metric), one JSON line on rank 0.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
 
 Workloads (BASELINE.json `configs`, SURVEY.md §8d):
   dual_system    configs[3] (DEFAULT -- the configuration the metric is quoted on): the full dual-system step for 64
@@ -13,7 +13,8 @@ Workloads (BASELINE.json `configs`, SURVEY.md §8d):
                  32-trajectory sample (8 per call).
 Multi-GPU: environments are independent, so every rank runs the same per-GPU workload on its own shard (weak scaling,
 no data-path collective; SURVEY.md §8e).  Timing: CUDA events on the launching stream, per timed step, L2 flushed
-between steps, max over ranks.
+between steps, max over ranks.  --dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy (float32;
+the inputs are seeded, so two builds of the library can be compared output for output).
 """
 import argparse
 import json
@@ -57,13 +58,14 @@ def peaks():
     if os.path.exists(p):
         with open(p) as fh:
             d = json.load(fh)
-        return dict(hbm=d.get("hbm_gbs", 6650.0), tf=d.get("bf16_tflops", 1590.0),
-                    tf_sustained=d.get("bf16_tflops_sustained", 1400.0), src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf=1590.0, tf_sustained=1400.0, src="fallback (B200_PROFILING.md)")
+        return dict(hbm=d.get("hbm_gbs", 3350.0), tf=d.get("bf16_tflops", 989.0),
+                    tf_sustained=d.get("bf16_tflops_sustained", 989.0), src="measured (MEASURED_PEAKS.json)")
+    # NVIDIA's data sheet for the H100 SXM at 700 W: 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s (never reached in practice)
+    return dict(hbm=3350.0, tf=989.0, tf_sustained=989.0, src="data sheet (H100 SXM, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -106,7 +108,7 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
-MIN_WARMUP = int(os.environ.get("N1_BENCH_MIN_WARMUP", "3"))  # profiling runs under ncu lower this; timed runs keep >= 3
+MIN_WARMUP = int(os.environ.get("N1_BENCH_MIN_WARMUP", "3"))  # profiling runs lower this; timed runs keep >= 3
 
 
 def host_threads():
@@ -172,16 +174,6 @@ def _gemm_classes(shapes, wl, world_B):
     return out
 
 
-def _traffic_table():
-    """ncu dram__bytes_read.sum + dram__bytes_write.sum per launch of named GEMM shapes, from committed captures
-    (profiles/r2_gemm_traffic.json: {"MxNxK": {"bytes": ..., "source": "profiles/..."}}); absent -> traffic null."""
-    p = os.path.join(ROOT, "profiles", "r2_gemm_traffic.json")
-    if os.path.exists(p):
-        with open(p) as fh:
-            return json.load(fh)
-    return {}
-
-
 def build_dual(dev, wl, rank):
     """Random-init InternVLA-N1 (Qwen2.5-VL-7B shapes + NavDP) and one step's synthetic inputs."""
     import numpy as np
@@ -210,6 +202,68 @@ def build_dual(dev, wl, rank):
         nz=torch.randn(wl["K"] - 1, B * wl["Ns"], wl["T"], 3, generator=g).pin_memory())
     grids = [list(wl["grid"])] * B
     return model, prompts, grids, host
+
+
+# ------------------------------------------------------------------------------------------------ --dump-outputs
+_LAST = [None]           # what the most recent call of a timed step returned
+DUMP_BUDGET = 60 * 1000 * 1000   # bytes of array data per run, all arrays together (files stay under 64 MB)
+
+
+def _named_arrays(x, name="out"):
+    """Flatten what a timed step returned into (name, tensor) pairs.  A tuple / list gives one array per member; a dict gives
+    one array per key, and a dict VALUE that is itself a dict of tensors (parameters, gradients) becomes one array: its
+    members flattened and concatenated in key order."""
+    if torch.is_tensor(x):
+        return [(name, x.detach().reshape(-1) if x.dim() == 0 else x.detach())]
+    if isinstance(x, (int, float)):
+        return [(name, torch.tensor([float(x)]))]
+    if isinstance(x, dict):
+        out = []
+        for k, v in x.items():
+            if isinstance(v, dict):
+                out.append((str(k), [t.detach().reshape(-1) for _, t in sorted(v.items())]))
+            else:
+                out += _named_arrays(v, str(k))
+        return out
+    if isinstance(x, (tuple, list)):
+        return [p for i, v in enumerate(x) for p in _named_arrays(v, "%s%d" % (name, i))]
+    return []
+
+
+def dump_outputs(args, rank, result):
+    """--dump-outputs DIR: the arrays the timed path returned in its last timed step, as DIR/<name>.npy in float32, at most
+    64 MB in all.  Small arrays are written whole; what is left of the budget is shared by the large ones, each stored as
+    every stride-th element from a seeded offset (same indices every run)."""
+    if not args.dump_outputs or rank != 0:
+        return
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    arrays = _named_arrays(result)
+    if not arrays:
+        raise SystemExit("--dump-outputs: the timed step of workload %s returned no array" % args.workload)
+    size = lambda t: sum(p.numel() for p in t) if isinstance(t, list) else t.numel()
+    arrays.sort(key=lambda nt: size(nt[1]))
+    left = DUMP_BUDGET // 4
+    rng = np.random.Generator(np.random.PCG64(2024))
+    for i, (name, t) in enumerate(arrays):
+        share = left // (len(arrays) - i)
+        n = size(t)
+        stride = max(1, -(-n // max(share, 1)))
+        off = int(rng.integers(stride))
+        parts = t if isinstance(t, list) else [t.reshape(-1)]
+        if stride > 1:   # one global stride over the concatenation, applied part by part
+            picked, pos = [], 0
+            for p in parts:
+                first = (off - pos) % stride
+                picked.append(p[first::stride])
+                pos += p.numel()
+            parts = picked
+        a = torch.cat([p.float() for p in parts]).cpu().numpy().astype(np.float32)
+        if not isinstance(t, list) and stride == 1:
+            a = a.reshape(tuple(t.shape))
+        left -= a.size
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------ our arm
@@ -250,7 +304,7 @@ def _finish(args, wl, world, rank, dev, ms, ms_e2e, launches, clocks, prof, B, e
         "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, MIN_WARMUP), "ms_per_step": ms_per_step,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "impl": "ours", "config": cfg, "e2e": e2e, "gpu_launches": int(launches["total_launches"]), "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "n1::gemm_kernel<BN> (tcgen05, all GEMM launches of one step)",
+        "roofline": {"bound": "tensor", "kernel": "n1::gemm_kernel<BN> (wgmma, all GEMM launches of one step)",
                      "achieved": achieved_tf, "peak": peak, "unit": "TFLOP/s", "frac": achieved_tf / peak,
                      "traffic": None, "peak_source": pk["src"] + (" sustained" if ms_per_step > 50 else " burst"),
                      "gemm_launches_per_step": int(prof["gemm_launches"]), "gemm_ms_per_step": prof["gemm_ms"],
@@ -263,14 +317,13 @@ def _finish(args, wl, world, rank, dev, ms, ms_e2e, launches, clocks, prof, B, e
         fl = (4.0 if dom["N"] < 0 else 2.0) * dom["M"] * abs(dom["N"]) * dom["K"]
         per_ms = dom["ms"] / dom["count"]
         key = "%dx%dx%d" % (dom["M"], abs(dom["N"]), dom["K"])
-        tr = _traffic_table().get(key)
         fam = dict(out["roofline"])
         a_tf = fl / (per_ms * 1e-3) / 1e12
         pk1 = pk["tf"]   # a single launch is short: the burst figure is the denominator
-        out["roofline"] = {"bound": "tensor", "kernel": "n1::gemm_kernel<BN,CM> (tcgen05) M x N x K = %s, %d launches per step"
+        out["roofline"] = {"bound": "tensor", "kernel": "n1::gemm_kernel<BN> (wgmma) M x N x K = %s, %d launches per step"
                                                          % (key, dom["count"]),
                            "achieved": a_tf, "peak": pk1, "unit": "TFLOP/s", "frac": a_tf / pk1,
-                           "traffic": tr["bytes"] if tr else None, "traffic_source": tr["source"] if tr else None,
+                           "traffic": None,
                            "algorithmic_bytes": 2.0 * (dom["M"] * dom["K"] + abs(dom["N"]) * dom["K"] + dom["M"] * abs(dom["N"])
                                                        // (2 if abs(dom["N"]) == 37888 else 1)),
                            "us_per_launch": per_ms * 1e3, "ms_per_step": dom["ms"],
@@ -303,7 +356,7 @@ def _finish(args, wl, world, rank, dev, ms, ms_e2e, launches, clocks, prof, B, e
 
 def _timing_tools(dev, world):
     import torch.distributed as dist
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -318,14 +371,14 @@ def _timing_tools(dev, world):
             if use_events:
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 a.record()
-                fn()
+                _LAST[0] = fn()
                 b.record()
                 b.synchronize()
                 tot += a.elapsed_time(b)
             else:  # includes host work (D2H + numpy tail): wall clock around a synchronised region
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                fn()
+                _LAST[0] = fn()
                 torch.cuda.synchronize()
                 tot += (time.perf_counter() - t0) * 1e3
         return tot
@@ -337,7 +390,7 @@ def run_ours_dual(args, wl):
     from internnav_b200 import _lib
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs an H100: there is no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -370,6 +423,7 @@ def run_ours_dual(args, wl):
     barrier()
     with ClockSampler(local) as clk:
         ms = timed(step_resident, args.steps)
+    dump_outputs(args, rank, _LAST[0])
     barrier()
     launches = _lib.prof_read()
     launches["total_launches"] //= max(args.steps, 1)
@@ -448,7 +502,7 @@ def run_ours_s2(args, wl):
     from internnav_b200.qwen import QWEN25VL_7B, System2
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs an H100: there is no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -480,6 +534,7 @@ def run_ours_s2(args, wl):
     barrier()
     with ClockSampler(local) as clk:
         ms = timed(step_resident, args.steps)
+    dump_outputs(args, rank, _LAST[0])
     barrier()
     launches = _lib.prof_read()
     launches["total_launches"] //= max(args.steps, 1)
@@ -538,7 +593,7 @@ def run_ours_train(args, wl):
     from internnav_b200.train_step import DualSystemTrainer
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs an H100: there is no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -571,7 +626,8 @@ def run_ours_train(args, wl):
         loss = tr.step(b, n, t)
         if world > 1:
             exch.append(tr.exchange_ms())
-        return loss
+        # what a caller of the step holds afterwards: the loss, the reduced gradients and the updated fp32 masters
+        return {"loss": loss, "grads": dict(tr.buckets.grads), "params": dict(tr.masters)}
 
     def step_e2e():
         it[0] += 1
@@ -585,6 +641,7 @@ def run_ours_train(args, wl):
     barrier()
     with ClockSampler(local) as clk:
         ms = timed(step_resident, args.steps)
+    dump_outputs(args, rank, _LAST[0])
     barrier()
     launches = _lib.prof_read()
     launches["total_launches"] //= max(args.steps, 1)
@@ -653,7 +710,7 @@ def run_ours_denoise(args, wl):
 
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs an H100: there is no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -670,7 +727,7 @@ def run_ours_denoise(args, wl):
     h_x0 = torch.randn(R, T, 3, generator=g).pin_memory()
     h_nz = torch.randn(K - 1, R, T, 3, generator=g).pin_memory()
     d_goal, d_rgbd, d_x0, d_nz = (t.to(dev) for t in (h_goal, h_rgbd, h_x0, h_nz))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def step_resident():
         return model.sample(d_goal, d_rgbd, d_x0, d_nz, num_steps=K)
@@ -696,14 +753,14 @@ def run_ours_denoise(args, wl):
             if use_events:
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 a.record()
-                fn()
+                _LAST[0] = fn()
                 b.record()
                 b.synchronize()
                 tot += a.elapsed_time(b)
             else:  # includes host work (D2H + numpy tail): wall clock around a synchronised region
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                fn()
+                _LAST[0] = fn()
                 torch.cuda.synchronize()
                 tot += (time.perf_counter() - t0) * 1e3
         return tot
@@ -714,6 +771,7 @@ def run_ours_denoise(args, wl):
     barrier()
     with ClockSampler(local) as clk:
         ms = timed(step_resident, args.steps)
+    dump_outputs(args, rank, _LAST[0])
     barrier()
     launches = _lib.prof_read()
     clocks = clk.summary()
@@ -723,7 +781,7 @@ def run_ours_denoise(args, wl):
     ms_e2e = timed(step_e2e, args.steps, use_events=False)
     barrier()
 
-    # roofline pass for the dominant kernel (tcgen05 GEMM): per-launch CUDA events, NOT part of the timed runs above;
+    # roofline pass for the dominant kernel (wgmma GEMM): per-launch CUDA events, NOT part of the timed runs above;
     # eager launches here (the timed runs replay the same launch sequence from a CUDA graph)
     _lib.prof_read()
     _lib.prof_enable(True)
@@ -762,7 +820,7 @@ def run_ours_nextdit(args, wl):
 
     rank, world, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs an H100: there is no CPU path")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -797,14 +855,14 @@ def run_ours_nextdit(args, wl):
             if use_events:
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 a.record()
-                fn()
+                _LAST[0] = fn()
                 b.record()
                 b.synchronize()
                 tot += a.elapsed_time(b)
             else:
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                fn()
+                _LAST[0] = fn()
                 torch.cuda.synchronize()
                 tot += (time.perf_counter() - t0) * 1e3
         return tot
@@ -815,6 +873,7 @@ def run_ours_nextdit(args, wl):
     barrier()
     with ClockSampler(local) as clk:
         ms = timed(step_resident, args.steps)
+    dump_outputs(args, rank, _LAST[0])
     barrier()
     launches = _lib.prof_read()
     clocks = clk.summary()
@@ -1060,10 +1119,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "eager"])
     ap.add_argument("--workload", default="dual_system", choices=sorted(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true", help="skip the same-GPU PyTorch-eager baseline leg (N = 1)")
     ap.add_argument("--batch", type=int, default=0, help="--impl eager: environments per call (default: the workload's)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs is implemented for --impl ours only")
     _claim_stdout()
     wl = WORKLOADS[args.workload]
     if args.impl == "eager":

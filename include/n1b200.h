@@ -1,4 +1,4 @@
-/* n1b200 -- C ABI of the B200-native InternVLA-N1 policy forward (libn1b200.so).
+/* n1b200 -- C ABI of the H100-native InternVLA-N1 policy forward (libn1b200.so).
  *
  * The reference (InternRobotics/InternNav) has no FFI seam on this path: the boundary is three nested Python
  * interfaces (SURVEY.md §8b).  This header is the C ABI placed *underneath* them; every entry point cites the
@@ -13,7 +13,7 @@
  *   - return value: 0 = OK, < 0 = error (message via n1_last_error, thread-local); no exceptions cross the ABI;
  *   - a handle is immutable after n1_load_*; concurrent calls from different host threads are safe iff each call uses
  *     its own workspace and stream (the reference drives S2 and S1 from two threads: internvla_n1_agent.py L133-208).
- *   - there is NO CPU fallback: every entry point fails with N1_ERR_NO_DEVICE when no sm_100 device is usable.
+ *   - there is NO CPU fallback: every entry point fails with N1_ERR_NO_DEVICE when no sm_90 device is usable.
  */
 #ifndef N1B200_H_
 #define N1B200_H_
@@ -76,7 +76,7 @@ typedef struct {
 
 /* ------------------------------------------------------------------------------------------------ lifecycle */
 const char* n1_version(void);
-int n1_device_ok(int device);                 /* 1 if `device` is an sm_100 GPU this library can drive */
+int n1_device_ok(int device);                 /* 1 if `device` is an sm_90 GPU this library can drive */
 int n1_create(n1_handle* out, int device);
 void n1_destroy(n1_handle h);
 const char* n1_last_error(void);              /* thread-local message of the last failing call */
@@ -228,8 +228,7 @@ int n1_resize_coeffs(int in_size, int out_size, int capacity_k, int32_t* bounds_
 /* ------------------------------------------------------------------------------------------------ training: backward primitives
  * First version of the backward kernels of the training branch (internvla_n1.py L58-318; navdp.py L291-312), exposed
  * one primitive at a time for parity tests against oracle/navdp_backward.py / oracle/qwen_backward.py.
- * STATUS: compiled for sm_100a, not yet validated on a B200 (written after the round's GPU budget was spent); nothing on
- * the inference path uses them.  All pointers are device pointers; activations bf16, parameter gradients fp32. */
+ * Nothing on the inference path uses them (tests/test_bwd_ops_gpu.py checks them against autograd).  All pointers are device pointers; activations bf16, parameter gradients fp32. */
 /* Training branch, System-1 side: tokens of the frozen RGB ViT (final norm, cls dropped, former_pe added) written into
  * the first frames*256 rows of every environment of mem bf16 [B, 2*frames*256, 384]; rgb fp32 [B, frames, 224, 224, 3]. */
 size_t n1_rgb_tokens_workspace_bytes(n1_handle h, int B);
@@ -334,8 +333,8 @@ int n1_op_attention(const void* q, const void* k, const void* v, void* o, int ld
                     const int32_t* cu_k, int max_seq_q, int kv_div, int causal, float scale, void* stream);
 
 /* Var-len self-attention (cu_seqlens int32 [batch + 1] on the device, q / k / v packed with row strides) with the row count
- * of the buffers given: head_dim 128 and <= 320 tokens per sequence run on the tcgen05 kernel (Q K^T and P V on
- * tcgen05.mma, scores in tensor memory, TMA-loaded tiles) -- the decoder prefill attention of generate_latents
+ * of the buffers given: head_dim 128 and <= 320 tokens per sequence run on the wgmma kernel (Q K^T and P V on
+ * wgmma, scores in registers, TMA-loaded tiles) -- the decoder prefill attention of generate_latents
  * (internvla_n1.py L206 / L338; flash_attention_2 in the reference, internvla_n1_policy.py L36).  *used_tcgen05 reports
  * which kernel ran (N1_ATTN_TC=0 forces the mma.sync kernel). */
 int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int ldq, int ldk, int ldv, int ldo, int heads_q,

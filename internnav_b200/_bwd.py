@@ -1,6 +1,6 @@
 """ctypes bindings of the backward primitives (include/n1b200.h, "training: backward primitives").
 
-Validated on the B200 against PyTorch autograd / torch.optim (tests/test_bwd_ops_gpu.py, profiles/r2_bwd_ops_parity.log);
+Validated on the H100 against PyTorch autograd / torch.optim (tests/test_bwd_ops_gpu.py);
 used by the training step (train_s1.py, train_step.py).  Nothing on the inference path imports this module.
 """
 import ctypes

@@ -1,6 +1,6 @@
 """ctypes binding of libn1b200.so (include/n1b200.h).  PyTorch is used for device memory and streams only.
 
-There is deliberately no fallback: if the shared library is missing, or no sm_100 device is present when a
+There is deliberately no fallback: if the shared library is missing, or no sm_90 device is present when a
 compute entry point is called, the call raises.
 """
 import ctypes
@@ -90,7 +90,7 @@ def lib():
         if _lib is None:
             if not os.path.exists(LIB_PATH):
                 raise ImportError(
-                    "%s not found: build it with `python -m internnav_b200.build` (nvcc, sm_100a). "
+                    "%s not found: build it with `python -m internnav_b200.build` (nvcc, sm_90a). "
                     "There is no CPU/PyTorch fallback for the n1b200 hot path." % LIB_PATH)
             L = ctypes.CDLL(LIB_PATH)
             for name, (res, args) in SYMBOLS.items():
@@ -237,7 +237,7 @@ def attention(q, k, v, heads_q, heads_kv, head_dim, batch, seq_q, seq_k, cu_q=No
 
 def attention_varlen(q, k, v, heads_q, heads_kv, head_dim, cu_seqlens, max_seq, causal=True, scale=None):
     """Var-len self-attention over packed rows (q / k / v: views with unit inner stride, `cu_seqlens` int32 [batch + 1]).
-    -> (o [rows, heads_q * hd], used_tcgen05: whether the tcgen05 kernel ran)."""
+    -> (o [rows, heads_q * hd], used_tcgen05: whether the wgmma kernel ran)."""
     assert q.dtype == torch.bfloat16 and q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1
     o = torch.empty(q.shape[0], heads_q * head_dim, device=q.device, dtype=torch.bfloat16)
     if scale is None:
@@ -251,7 +251,7 @@ def attention_varlen(q, k, v, heads_q, heads_kv, head_dim, cu_seqlens, max_seq, 
 
 
 def ff_block(x, ln_w, ln_b, w1, b1, w2, b2, eps=1e-5, out=None, cluster=2):
-    """out = x + gelu(LayerNorm(x) @ w1.T + b1) @ w2.T + b2 (NavDP decoder FF block, residual stream in tensor memory)."""
+    """out = x + gelu(LayerNorm(x) @ w1.T + b1) @ w2.T + b2 (NavDP decoder FF block, one fused kernel)."""
     assert x.dtype == torch.bfloat16 and x.shape[1] == 384 and w1.shape == (1536, 384) and w2.shape == (384, 1536)
     assert w1.is_contiguous() and w2.is_contiguous() and x.stride(1) == 1
     if out is None:

@@ -1,8 +1,8 @@
-"""Build libn1b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libn1b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m internnav_b200.build [--force]
 
-The shared library is the C-ABI product (include/n1b200.h); it is git-ignored but travels to the GPU box.
+The shared library is the C-ABI product (include/n1b200.h); it is a build product and is not committed.
 """
 import hashlib
 import os
@@ -17,7 +17,7 @@ OBJ = os.path.join(HERE, "_build")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -57,7 +57,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

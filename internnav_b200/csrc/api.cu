@@ -55,7 +55,7 @@ void require_device(int device) {
   if (device < 0 || device >= n) throw Error(N1_ERR_NO_DEVICE, "device index out of range");
   cudaDeviceProp p;
   N1_CUDA(cudaGetDeviceProperties(&p, device));
-  if (p.major != 10) throw Error(N1_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(p.major) + std::to_string(p.minor) + "; n1b200 kernels are sm_100a only");
+  if (p.major != 9) throw Error(N1_ERR_NO_DEVICE, std::string("device is sm_") + std::to_string(p.major) + std::to_string(p.minor) + "; n1b200 kernels are sm_90a only");
 }
 
 void use(n1_handle h) {
@@ -85,7 +85,7 @@ inline bf16* B16(void* p) { return static_cast<bf16*>(p); }
 
 extern "C" {
 
-const char* n1_version(void) { return "n1b200 0.1 (sm_100a)"; }
+const char* n1_version(void) { return "n1b200 0.1 (sm_90a)"; }
 
 const char* n1_last_error(void) { return g_err.c_str(); }
 
@@ -630,7 +630,7 @@ int n1_op_attention(const void* q, const void* k, const void* v, void* o, int ld
 }
 
 /* n1_op_attention with the row count of the packed buffers: lets var-len self-attention with head_dim 128 and <= 320
- * tokens per sequence take the tcgen05 kernel (attention_tc.cu), which addresses q / k / v through TMA tensor maps */
+ * tokens per sequence take the wgmma kernel (attention_wgmma.cu), which addresses q / k / v through TMA tensor maps */
 int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int ldq, int ldk, int ldv, int ldo, int heads_q,
                        int heads_kv, int head_dim, int batch, const int32_t* cu_seqlens, int max_seq, int64_t total_rows,
                        int causal, float scale, int* used_tcgen05, void* stream) {

@@ -12,7 +12,7 @@
 // Flash-attention style: a CTA owns 64 query rows of one (sequence, head); 4 warps x 16 rows; K/V streamed in
 // 64-key tiles through a 2-stage cp.async ring; S = QK^T and O += PV on mma.sync.m16n8k16 (bf16, fp32 accumulate)
 // with ldmatrix operand fetch; online softmax in registers with quad shuffles.
-// The hd-128 var-len prefill of up to 320 tokens per sequence is routed to the tcgen05 kernel (attention_tc.cu) by
+// The hd-128 var-len prefill of up to 320 tokens per sequence is routed to the wgmma kernel (attention_wgmma.cu) by
 // attention(); this file keeps the general path (any length, GQA, slotted K/V cache, head_dim 48 / 64 / 80 / 128).
 #include <stdlib.h>
 
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
 // the Q-former self-attention and the goal compressor.  One CTA per query sequence, one warp per head.  Q, K, V rows
 // (all heads, contiguous in memory) are staged with fully coalesced 16-byte cp.async; each warp runs QK^T, a
 // single-pass softmax and PV for its head on mma.sync; O is staged back through the Q tile and written coalesced.
-// The generic kernel above spent 4x the work on padding at these shapes (profiles/r1_ncu_small_v0_summary.txt).
+// The generic kernel above spent 4x the work on padding at these shapes.
 template <int NKP>  // key tiles of 16
 __global__ void __launch_bounds__(256) attn_small_kernel(const AttnParams p, const int G) {
   constexpr int HD = 48;

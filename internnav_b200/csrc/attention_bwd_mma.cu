@@ -10,7 +10,7 @@
 //   phase 3  per 16-key block (one warp):  dV = P^T dO,  dK = (P o (dP - D))^T Q * scale              -> global fp32
 // S = Q K^T is therefore formed three times (7 matmuls instead of the minimal 5) -- in exchange no atomics, no cross-warp
 // reductions and a deterministic result.  All products run on mma.sync.m16n8k16 (bf16 operands, fp32 accumulate) with
-// ldmatrix operand fetch: the tiles are 16 x 32 per warp, far below what a tcgen05 128-row MMA needs, and the whole
+// ldmatrix operand fetch: the tiles are 16 x 32 per warp, far below what a 64-row wgmma needs, and the whole
 // backward of the depth ViT is ~1.6 TFLOP per step.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Backward primitives of the training step.  See bwd_kernels.h (status: compiled, not yet run on a B200).
+// Backward primitives of the training step.  See bwd_kernels.h.
 // Specification: oracle/navdp_backward.py (lin_bwd, ln_bwd, gelu_bwd, attn_core_bwd, ...) and oracle/qwen_backward.py.
 #include "bwd_kernels.h"
 
@@ -225,8 +225,7 @@ constexpr int AQ = 8;  // query rows per tile
 // share the K/V sequence (kv_div), the query heads of the GQA group and the query tiles.  128 threads.
 // `stage`: K and V of the head are first copied into shared memory (bf16, rows padded by one word): every pass below reads
 // them ~(query heads of the group) x (query tiles) times, and the score / dP passes walk them one key per thread -- from
-// global memory those are 2-byte loads 32 rows apart (profiles/r2_launches_ddp_train_v1_summary.txt: 2.5 ms per launch in the
-// System-2 backward, 7 query heads x 304 keys x 128).
+// global memory those are 2-byte loads 32 rows apart.
 __global__ void __launch_bounds__(128) attn_bwd_kernel(const AttnBwdParams p, const int stage) {
   extern __shared__ float sm[];
   const AttnParams& f = p.f;

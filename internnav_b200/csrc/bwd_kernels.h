@@ -1,10 +1,8 @@
 // Backward primitives of the training step (SURVEY.md §8 row a13) -- first version, CUDA-core kernels written for
 // correctness against oracle/navdp_backward.py and oracle/qwen_backward.py (the hand-written backward specs), not yet
-// for speed; the matrix products of the backward (dgrad, wgrad) go through the tcgen05 GEMM on transposed operands.
+// for speed; the matrix products of the backward (dgrad, wgrad) go through the wgmma GEMM on transposed operands.
 //
-// STATUS: written at the end of round 1 without GPU time left -- compiled for sm_100a, NOT yet run on a B200.  Nothing
-// on the inference path calls into this file; the op-level tests (tests/test_bwd_ops_gpu.py) are skipped until a parity
-// run is on record.
+// Nothing on the inference path calls into this file; tests/test_bwd_ops_gpu.py checks every primitive against autograd.
 #pragma once
 #include "n1_ops.h"
 

@@ -1,30 +1,23 @@
-// FF block of the NavDP decoder layer as ONE kernel, residual stream resident in tensor memory:
+// FF block of the NavDP decoder layer as ONE kernel, hidden activations never leaving the SM:
 //
 //     x  <-  x + W2 · GELU(W1 · LayerNorm(x) + b1) + b2            (D = 384, F = 1536; navdp.py L57-66: norm3 / linear1 /
 //                                                                    exact GELU / linear2 / residual of the pre-norm layer)
 //
 // replaces three launches (LayerNorm, FF1+GELU GEMM, FF2+residual GEMM) and the HBM round trips of the [rows, 384]
-// normalised input and the [rows, 1536] hidden.  Per CTA, one 128-row tile at a time (persistent over tiles):
+// normalised input and the [rows, 1536] hidden.  Per CTA, one 64-row tile at a time (persistent over tiles):
 //
-//   prologue (16 epilogue warps, thread = one row x 96 columns): x rows from global -> LayerNorm -> bf16 A operand in SMEM
-//       (128-byte swizzled K-major, 96 KB) AND  x + b2  in fp32 into TMEM columns 0..383 (tcgen05.st): the second GEMM
-//       then ACCUMULATES into the residual stream, so the residual add and the output bias cost no epilogue work;
-//   hidden chunks of 128 columns:  H_j = LN(x) · W1[128j:128j+128]^T  (tcgen05.mma M128 N128 into TMEM 384..511)
-//       -> all 16 epilogue warps: tcgen05.ld (32 columns each), + b1, GELU (packed f32x2 polynomial, no MUFU), bf16,
-//          swizzled SMEM chunk  ->  x_tmem += H_j · W2[:, 128j:128j+128]^T   (2 x M128 N192 per k-step);
-//       one TMEM and one SMEM chunk buffer: GEMM1(j+1) runs while chunk j is in the GELU epilogue, GEMM2(j) while chunk
-//       j+1 is.  (The first version used 64-column chunks, double buffered: its 768 small MMAs per tile made the single
-//       issuing thread the limiter -- tensor pipe 25 % active, no barrier ever waited on, profiles/r2_ncu_ff_block_v0_*.)
-//   TWO MMA-issuing warps (GEMM1 and GEMM2 each have their own issuer, TMA producer and weight ring): one thread can
-//       issue a tcgen05.mma only every ~100-150 cycles (descriptor moves into uniform registers), which is longer than an
-//       N = 128 / N = 192 MMA occupies the tensor pipe (64 / 96 cycles) -- with one issuer (v1) the pipe was 30 % busy;
-//   W1 streams through a 3 x 16 KB ring, W2 through a 2 x 24 KB ring; CM = 2: the two CTAs of a cluster fetch half a slice
-//       each and multicast it;
-//   final epilogue: TMEM 0..383 -> bf16 -> SMEM staging -> TMA store to x (in place).
-//
-// Differences from the first fused MLP of round 1 (removed): LayerNorm inside, residual in TMEM, 16
-// epilogue warps instead of 8 (the GELU epilogue was the limiter: 2 warps per scheduler could not hide FMA latency), and
-// a MUFU-free GELU in packed fp32.
+//   warps 8, 9      producers: warp 8 streams W1 through a 3 x 16 KB ring (one [128 x 64] k-block of a hidden chunk per
+//                   slot), warp 9 streams W2 through a 2 x 48 KB ring (one [384 x 64] k-block per slot).  CM = 2: the two
+//                   CTAs of a cluster work on neighbouring row tiles, fetch half of every slot each and multicast it.
+//   warpgroups 0-1  consumers (320 threads leave them 204 registers each), both on the same 64 rows:
+//       prologue    x rows -> LayerNorm -> bf16 A operand in shared memory (128-byte swizzled K-major, 48 KB);
+//       per hidden chunk of 128 columns: warpgroup g computes its 64 columns  H = LN(x) · W1[128 j + 64 g ..]^T  (wgmma
+//                   m64n64k16, fp32 registers), adds b1, GELU, and writes them as bf16 into the swizzled chunk buffer
+//                   (double buffered); after one barrier both read the whole chunk back as the A operand of
+//                   y[:, 192 g .. 192 g + 192] += GELU(H) · W2[192 g .., chunk]^T  (m64n192k16: the output columns are
+//                   split over the warpgroups, 96 accumulator registers each).  GEMM2 of chunk j stays in flight under
+//                   GEMM1 of chunk j + 1, and one warpgroup's GELU runs under the other's MMAs;
+//       epilogue    y + x + b2 -> bf16 -> global (in place: a thread re-reads exactly the elements it overwrites).
 #include <stdlib.h>
 
 #include <mutex>
@@ -35,16 +28,16 @@
 namespace n1 {
 namespace {
 
-constexpr int D = 384, F = 1536, BM = 128, HC = 128;
+constexpr int D = 384, F = 1536, BM = 64, HC = 128;
 constexpr int NCH = F / HC;                          // 12 hidden chunks
-constexpr int kS1 = 3, kS1Bytes = 16384;             // W1 ring: one k-block [128 x 64] of a hidden chunk per slot
-constexpr int kS2 = 2, kS2Bytes = 24576;             // W2 ring: one N-half [192 x 64] of a k-block per slot
-constexpr int kABytes = BM * D * 2;                  // 98304: 6 k-blocks of [128 x 64]
-constexpr int kHBytes = BM * HC * 2;                 // 32768: the GELU(H) chunk, 2 k-blocks of [128 x 64]
-constexpr int kEpiWarps = 16;
-constexpr int kThreads = 128 + 32 * kEpiWarps;       // 640: 2 TMA producers, 2 MMA issuers, 16 epilogue warps
-constexpr int kStatBytes = 128 * 2 * 4;              // LayerNorm statistics of the tile: [128 rows][mean, rstd]
-constexpr int kSmem = kABytes + kHBytes + kS1 * kS1Bytes + kS2 * kS2Bytes + kStatBytes + 512 + 1024;
+constexpr int kS1 = 3, kS1Bytes = HC * 64 * 2;       // W1 ring: one k-block [128 x 64] of a hidden chunk per slot
+constexpr int kS2 = 2, kS2Bytes = D * 64 * 2;        // W2 ring: one k-block [384 x 64] of a hidden chunk per slot
+constexpr int kABytes = BM * D * 2;                  // 49152: 6 k-blocks of [64 x 64]
+constexpr int kHBytes = BM * HC * 2;                 // 16384: one GELU(H) chunk, 2 k-blocks of [64 x 64]
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * kConsumerWarps + 64;  // 320
+constexpr int kSmem = kABytes + 2 * kHBytes + kS1 * kS1Bytes + kS2 * kS2Bytes + 256 + 1024;
+static_assert(kSmem <= 232448, "ff_block: shared memory budget (227 KB per block)");
 
 struct FfArgs {
   int M;
@@ -56,83 +49,47 @@ struct FfArgs {
   float eps;
   const float* b1;
   const float* b2;
+  bf16* out;
+  int ldo;
 };
 
-// erf(u / sqrt 2) ~= u P(u^2) on |u| <= 4: least-squares fit weighted for the GELU product, scaled by (1 - 1e-4) so that
-// |u P(u^2)| < 1 everywhere and no clamp of the result is needed.  |gelu error| <= 3e-4 for |x| <= 4 and <= 4e-5 |x|
-// beyond (a fraction of a bf16 ulp of the result).  Packed fp32: two values per instruction, no MUFU.
-__device__ __forceinline__ float2 gelu2(float2 x) {
-  const float2 u = make_float2(fminf(fmaxf(x.x, -4.0f), 4.0f), fminf(fmaxf(x.y, -4.0f), 4.0f));
-  const float2 s = __fmul2_rn(u, u);
-  float2 p = __ffma2_rn(make_float2(4.477657000734325e-08f, 4.477657000734325e-08f), s,
-                        make_float2(-3.1557883630739525e-06f, -3.1557883630739525e-06f));
-  p = __ffma2_rn(p, s, make_float2(9.507098729955032e-05f, 9.507098729955032e-05f));
-  p = __ffma2_rn(p, s, make_float2(-0.001619840506464243f, -0.001619840506464243f));
-  p = __ffma2_rn(p, s, make_float2(0.01750575192272663f, 0.01750575192272663f));
-  p = __ffma2_rn(p, s, make_float2(-0.12906235456466675f, -0.12906235456466675f));
-  p = __ffma2_rn(p, s, make_float2(0.7956569194793701f, 0.7956569194793701f));
-  const float2 e = __fmul2_rn(u, p);
-  const float2 h = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  return __ffma2_rn(h, e, h);
-}
+// barrier among the consumer warps only (named barrier 1; the producer warps never join it)
+__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory"); }
 
-// barrier among the 16 epilogue warps only (named barrier 1; the producer / MMA warps never join it)
-__device__ __forceinline__ void epi_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32) : "memory"); }
-
-// UI: the MMA warp runs its loop with all lanes and an elected lane issues (operands stay in uniform registers)
-template <int CM, bool UI>
-// 20 warps = 5 per scheduler: 16384 / (5 * 32) = 102 -> ptxas settles on 96 registers per thread
+template <int CM>
 __global__ void __launch_bounds__(kThreads, 1)
-ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
-                const __grid_constant__ CUtensorMap tmOut, const FfArgs args) {
+ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2, const FfArgs args) {
   constexpr uint16_t kMask = (1u << CM) - 1;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sH = smem + kABytes;
-  uint8_t* sW1 = sH + kHBytes;
+  uint8_t* sW1 = sH + 2 * kHBytes;
   uint8_t* sW2 = sW1 + kS1 * kS1Bytes;
-  float* sStat = reinterpret_cast<float*>(sW2 + kS2 * kS2Bytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sW2 + kS2 * kS2Bytes + kStatBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sW2 + kS2 * kS2Bytes);
   uint64_t* w1_full = bars;                // [3]
   uint64_t* w1_empty = bars + 3;           // [3]
   uint64_t* w2_full = bars + 6;            // [2]
   uint64_t* w2_empty = bars + 8;           // [2]
-  uint64_t* a_full = bars + 10;            // LN(x) operand written and x + b2 seeded in TMEM (16 warp arrivals)
-  uint64_t* hacc_full = bars + 11;         // GEMM1(j) complete -> TMEM H readable
-  uint64_t* hacc_empty = bars + 12;        // epilogue finished reading TMEM H (16 warp arrivals)
-  uint64_t* hs_full = bars + 13;           // SMEM H written (16 warp arrivals)
-  uint64_t* hs_empty = bars + 14;          // GEMM2 finished reading SMEM H
-  uint64_t* y_full = bars + 15;            // all MMAs of the tile complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = CM > 1 ? (int)cluster_ctarank() : 0;
   const int cluster_id = blockIdx.x / CM, num_clusters = gridDim.x / CM;
   const int super_m = (args.tiles_m + CM - 1) / CM;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmW1), tma_prefetch_desc(&tmW2), tma_prefetch_desc(&tmOut);
-    for (int s = 0; s < kS1; ++s) mbar_init(&w1_full[s], 1), mbar_init(&w1_empty[s], CM);
-    for (int s = 0; s < kS2; ++s) mbar_init(&w2_full[s], 1), mbar_init(&w2_empty[s], CM);
-    mbar_init(a_full, kEpiWarps);
-    mbar_init(hacc_full, 1), mbar_init(hacc_empty, kEpiWarps);
-    mbar_init(hs_full, kEpiWarps), mbar_init(hs_empty, 1);
-    mbar_init(y_full, 1);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmW1), tma_prefetch_desc(&tmW2);
+    // every consumer warp of every CTA of the cluster releases a slot (its halves live in all of them)
+    for (int s = 0; s < kS1; ++s) mbar_init(&w1_full[s], 1), mbar_init(&w1_empty[s], kConsumerWarps * CM);
+    for (int s = 0; s < kS2; ++s) mbar_init(&w2_full[s], 1), mbar_init(&w2_empty[s], kConsumerWarps * CM);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
+  // peers' barriers must be initialised before any multicast / remote arrive reaches them
   if (CM > 1) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer of W1 (GEMM1's ring)
-    if (lane == 0) {
+  if (warp >= kConsumerWarps) {
+    if (warp == kConsumerWarps && lane == 0) {
+      // ------------------------------------------------------------------ TMA producer of W1 (GEMM1's ring)
       int slot = 0;
       uint32_t ph = 0;
       for (int t = cluster_id; t < super_m; t += num_clusters)
@@ -144,127 +101,56 @@ ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant_
             if (CM == 1) {
               tma_load_2d(dst, &tmW1, &w1_full[slot], kb * 64, j * HC);
             } else {  // each CTA fetches 64 of the 128 rows and multicasts them
-              tma_load_2d_mc(dst + rank * 8192, &tmW1, &w1_full[slot], kb * 64, j * HC + rank * 64, kMask);
+              tma_load_2d_mc(dst + rank * (kS1Bytes / 2), &tmW1, &w1_full[slot], kb * 64, j * HC + rank * (HC / 2), kMask);
             }
             if (++slot == kS1) slot = 0, ph ^= 1;
           }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ TMA producer of W2 (GEMM2's ring)
-    if (lane == 0) {
+    } else if (warp == kConsumerWarps + 1 && lane == 0) {
+      // ------------------------------------------------------------------ TMA producer of W2 (GEMM2's ring)
       int slot = 0;
       uint32_t ph = 0;
       for (int t = cluster_id; t < super_m; t += num_clusters)
         for (int j = 0; j < NCH; ++j)
-          for (int kb = 0; kb < HC / 64; ++kb)
-            for (int nh = 0; nh < 2; ++nh) {  // W2[:, 128j + 64kb : +64), output rows [192nh, 192nh + 192)
-              mbar_wait(&w2_empty[slot], ph ^ 1);
-              mbar_arrive_expect_tx(&w2_full[slot], kS2Bytes);
-              uint8_t* dst = sW2 + slot * kS2Bytes;
-              if (CM == 1) {
-                tma_load_2d(dst, &tmW2, &w2_full[slot], j * HC + kb * 64, nh * 192);
-              } else {
-                tma_load_2d_mc(dst + rank * 12288, &tmW2, &w2_full[slot], j * HC + kb * 64, nh * 192 + rank * 96, kMask);
-              }
-              if (++slot == kS2) slot = 0, ph ^= 1;
+          for (int kb = 0; kb < HC / 64; ++kb) {  // W2[:, 128j + 64kb : +64) as two boxes of 192 output rows
+            mbar_wait(&w2_empty[slot], ph ^ 1);
+            mbar_arrive_expect_tx(&w2_full[slot], kS2Bytes);
+            uint8_t* dst = sW2 + slot * kS2Bytes;
+            if (CM == 1) {
+              tma_load_2d(dst, &tmW2, &w2_full[slot], j * HC + kb * 64, 0);
+              tma_load_2d(dst + kS2Bytes / 2, &tmW2, &w2_full[slot], j * HC + kb * 64, 192);
+            } else {
+              tma_load_2d_mc(dst + rank * (kS2Bytes / 2), &tmW2, &w2_full[slot], j * HC + kb * 64, rank * 192, kMask);
             }
-    }
-    __syncwarp();
-  } else if (warp == 2 || warp == 3) {
-    // ------------------------------------------------------------------ MMA issuers: warp 2 = GEMM1, warp 3 = GEMM2
-    if (UI || lane == 0) {
-      auto mma = [&](uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-        if (UI) umma_f16_elect(d, a, b, idesc, acc); else umma_f16(d, a, b, idesc, acc);
-      };
-      auto commit = [&](uint64_t* bar) { if (UI) umma_commit_elect(bar); else umma_commit(bar); };
-      auto release = [&](uint64_t* bar) {
-        if (CM == 1) commit(bar);
-        else if (UI) umma_commit_mc_elect(bar, kMask);
-        else umma_commit_mc(bar, kMask);
-      };
-      int slot = 0;
-      uint32_t wph = 0, tph = 0;
-      if (warp == 2) {
-        // GEMM1: TMEM[384..511] = LN(x) · W1 chunk^T, K = 384: 6 k-blocks x 4 k-steps of M128 N128 K16 per chunk
-        constexpr uint32_t idesc1 = umma_idesc_bf16(BM, HC);
-        uint32_t he_ph = 0;
-        for (int t = cluster_id; t < super_m; t += num_clusters) {
-          mbar_wait(a_full, tph);  // LN(x) is in shared memory
-          tph ^= 1;
-          tc_fence_after();
-          for (int j = 0; j < NCH; ++j) {
-            mbar_wait(hacc_empty, he_ph ^ 1);  // the epilogue holds the previous chunk in registers: TMEM H is free
-            he_ph ^= 1;
-            tc_fence_after();
-            for (int kb = 0; kb < D / 64; ++kb) {
-              mbar_wait(&w1_full[slot], wph);
-              tc_fence_after();
-              const uint64_t ad = umma_desc_sw128(smem_u32(sA + kb * 16384));
-              const uint64_t bd = umma_desc_sw128(smem_u32(sW1 + slot * kS1Bytes));
-#pragma unroll
-              for (int k = 0; k < 4; ++k) mma(tmem + 384, ad + 2 * k, bd + 2 * k, idesc1, (kb | k) != 0 ? 1u : 0u);
-              release(&w1_empty[slot]);
-              if (++slot == kS1) slot = 0, wph ^= 1;
-            }
-            commit(hacc_full);
+            if (++slot == kS2) slot = 0, ph ^= 1;
           }
-        }
-      } else {
-        // GEMM2: x_tmem[0..383] += GELU(H chunk) · W2 chunk^T, K = 128: 2 k-blocks x 2 N-halves x 4 k-steps of M128 N192
-        constexpr uint32_t idesc2 = umma_idesc_bf16(BM, 192);
-        uint32_t hs_ph = 0;
-        for (int t = cluster_id; t < super_m; t += num_clusters) {
-          mbar_wait(a_full, tph);  // x + b2 is seeded in TMEM columns 0..383
-          tph ^= 1;
-          tc_fence_after();
-          for (int j = 0; j < NCH; ++j) {
-            mbar_wait(hs_full, hs_ph);  // GELU(H_j) is in shared memory
-            hs_ph ^= 1;
-            tc_fence_after();
-            for (int kb = 0; kb < HC / 64; ++kb) {
-              const uint64_t ad = umma_desc_sw128(smem_u32(sH + kb * 16384));
-              for (int nh = 0; nh < 2; ++nh) {
-                mbar_wait(&w2_full[slot], wph);
-                tc_fence_after();
-                const uint64_t bd = umma_desc_sw128(smem_u32(sW2 + slot * kS2Bytes));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) mma(tmem + nh * 192, ad + 2 * k, bd + 2 * k, idesc2, 1u);
-                release(&w2_empty[slot]);
-                if (++slot == kS2) slot = 0, wph ^= 1;
-              }
-            }
-            commit(hs_empty);
-          }
-          commit(y_full);  // GEMM1's MMAs precede GEMM2(11) through the epilogue, so this covers the whole tile
-        }
-      }
     }
-    __syncwarp();
   } else {
-    // ------------------------------------------------------------------ 16 epilogue warps
-    const int ew = warp - 4;                 // 0..15
-    const int quarter = warp & 3;            // TMEM lane quarter this warp may access (hardware rule: warp id % 4)
-    const int sub = ew >> 2;                 // 0..3: which of the 4 warps of this quarter (= its 32-column slice of a chunk)
-    const int r_in_tile = quarter * 32 + lane;
-    const uint32_t lane_base = uint32_t(quarter * 32) << 16;
-    uint32_t hacc_phase = 0, hs_phase = 0, tphase = 0;
-    // bulk-store staging: 2 KB per warp inside the H buffers (idle between the tile's last GEMM2 and the next tile's first
-    // GELU write); all 16 warps pass epi_barrier() in the next prologue after draining their store reads, so no warp's
-    // GELU write can land on another warp's pending store
-    uint8_t* my_store = sH + ew * 2048;
+    // ------------------------------------------------------------------ 2 consumer warpgroups
+    const int cw = warp;                     // 0..7
+    const int g = cw >> 2;                   // warpgroup: hidden columns [64 g, +64) of a chunk, output columns [192 g, +192)
+    const int quad = lane & 3;
+    const int r0 = (cw & 3) * 16 + (lane >> 2);  // this thread's accumulator rows: r0 and r0 + 8
+    auto release = [&](uint64_t* bar) {      // called by lane 0 of every consumer warp
+      if (CM == 1) {
+        mbar_arrive(bar);
+      } else {
+#pragma unroll
+        for (int c = 0; c < CM; ++c) mbar_arrive_cluster(bar, c);
+      }
+    };
+    int s1 = 0, s2 = 0;
+    uint32_t ph1 = 0, ph2 = 0;
     for (int t = cluster_id; t < super_m; t += num_clusters) {
       const int tm = t * CM + rank;
-      const int row = tm * BM + r_in_tile;
-      const bool row_ok = row < args.M;
-      // ---- prologue, pass A: row statistics, one warp per row (8 rows per warp), coalesced 8-byte loads, two-pass variance.
-      // All 24 loads of the warp's 8 rows are issued before the first use (one memory round trip instead of eight) and the
-      // eight shuffle reductions advance in lock-step.
+      // every MMA of the previous tile has completed in both warpgroups: the A operand and the chunk buffers are free
+      consumer_barrier();
+      // ---- prologue: LayerNorm, one warp per row (8 rows per warp), coalesced 8-byte loads, two-pass variance.  All 24
+      // loads of the warp's 8 rows are issued before the first use and the shuffle reductions advance in lock-step.
       {
         uint2 q[8][3];
 #pragma unroll
         for (int rr = 0; rr < 8; ++rr) {
-          const long grow = (long)tm * BM + ew * 8 + rr;
+          const long grow = (long)tm * BM + cw * 8 + rr;
           const bf16* xr = args.x + grow * args.ldx;
 #pragma unroll
           for (int i = 0; i < 3; ++i)
@@ -298,169 +184,125 @@ ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant_
         for (int o = 16; o > 0; o >>= 1)
 #pragma unroll
           for (int rr = 0; rr < 8; ++rr) sq[rr] += __shfl_xor_sync(0xffffffffu, sq[rr], o);
-        if (lane < 8) {
-          float mu = s[0], v = sq[0];
 #pragma unroll
-          for (int rr = 1; rr < 8; ++rr)
-            if (lane == rr) mu = s[rr], v = sq[rr];
-          sStat[(ew * 8 + lane) * 2] = mu;
-          sStat[(ew * 8 + lane) * 2 + 1] = rsqrtf(v * (1.0f / D) + args.eps);
-        }
-      }
-      epi_barrier();
-      // ---- pass B: this thread's row, columns [sub * 96, sub * 96 + 96)
-      const float mean = sStat[r_in_tile * 2], rstd = sStat[r_in_tile * 2 + 1];
-      const bf16* xrow = args.x + (long)row * args.ldx + sub * 96;
-      // normalised row -> swizzled A operand; x + b2 -> TMEM (fp32) in three batches of 32 columns; the x chunks of batch
-      // b + 1 are in flight while batch b is processed
-      uint4 xq[2][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        xq[0][i] = row_ok ? __ldg(reinterpret_cast<const uint4*>(xrow + i * 8)) : make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-      for (int batch = 0; batch < 3; ++batch) {
-        if (batch + 1 < 3) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            xq[(batch + 1) & 1][i] = row_ok ? __ldg(reinterpret_cast<const uint4*>(xrow + (batch + 1) * 32 + i * 8))
-                                            : make_uint4(0u, 0u, 0u, 0u);
-        }
-        uint32_t seed[32];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int col = sub * 96 + batch * 32 + i * 8;
-          const uint4 q = xq[batch & 1][i];
-          const uint32_t w4[4] = {q.x, q.y, q.z, q.w};
-          const float4 lw0 = __ldg(reinterpret_cast<const float4*>(args.ln_w + col));
-          const float4 lw1 = __ldg(reinterpret_cast<const float4*>(args.ln_w + col + 4));
-          const float4 lb0 = __ldg(reinterpret_cast<const float4*>(args.ln_b + col));
-          const float4 lb1 = __ldg(reinterpret_cast<const float4*>(args.ln_b + col + 4));
-          const float4 c0 = __ldg(reinterpret_cast<const float4*>(args.b2 + col));
-          const float4 c1 = __ldg(reinterpret_cast<const float4*>(args.b2 + col + 4));
-          const float lw[8] = {lw0.x, lw0.y, lw0.z, lw0.w, lw1.x, lw1.y, lw1.z, lw1.w};
-          const float lb[8] = {lb0.x, lb0.y, lb0.z, lb0.w, lb1.x, lb1.y, lb1.z, lb1.w};
-          const float cb[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-          float v[8], y[8];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) v[2 * e] = bf16_lo(w4[e]), v[2 * e + 1] = bf16_hi(w4[e]);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            y[e] = (v[e] - mean) * rstd * lw[e] + lb[e];
-            seed[i * 8 + e] = __float_as_uint(v[e] + cb[e]);
-          }
+        for (int i = 0; i < 3; ++i) {
+          const int col = (lane + i * 32) * 4;
+          const float4 lw = __ldg(reinterpret_cast<const float4*>(args.ln_w + col));
+          const float4 lb = __ldg(reinterpret_cast<const float4*>(args.ln_b + col));
           // K-major, 128-byte swizzle: k-block col / 64, 16-byte chunk (col % 64) / 8 at position chunk ^ (row % 8)
           const int kb = col >> 6, ch = (col & 63) >> 3;
-          uint8_t* dst = sA + kb * 16384 + (r_in_tile >> 3) * 1024 + (r_in_tile & 7) * 128 + ((ch ^ (r_in_tile & 7)) << 4);
-          *reinterpret_cast<uint4*>(dst) = make_uint4(pack_bf16(y[0], y[1]), pack_bf16(y[2], y[3]), pack_bf16(y[4], y[5]),
-                                                      pack_bf16(y[6], y[7]));
+#pragma unroll
+          for (int rr = 0; rr < 8; ++rr) {
+            const float mu = s[rr], rstd = rsqrtf(sq[rr] * (1.0f / D) + args.eps);
+            const float y0 = (bf16_lo(q[rr][i].x) - mu) * rstd * lw.x + lb.x, y1 = (bf16_hi(q[rr][i].x) - mu) * rstd * lw.y + lb.y;
+            const float y2 = (bf16_lo(q[rr][i].y) - mu) * rstd * lw.z + lb.z, y3 = (bf16_hi(q[rr][i].y) - mu) * rstd * lw.w + lb.w;
+            // row cw * 8 + rr: 8-row group cw, row rr inside it
+            uint8_t* dst = sA + kb * 8192 + cw * 1024 + rr * 128 + ((ch ^ rr) << 4) + (col & 7) * 2;
+            *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(y0, y1), pack_bf16(y2, y3));
+          }
         }
-        tmem_st32(tmem + lane_base + sub * 96 + batch * 32, seed);
       }
-      tmem_st_wait();
       fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive_elect(a_full);
+      consumer_barrier();
 
-      // ---- hidden chunks: every warp takes its 32 columns of every chunk
+      float y[96];
       for (int j = 0; j < NCH; ++j) {
-        mbar_wait(hacc_full, hacc_phase);
-        hacc_phase ^= 1;
-        tc_fence_after();
-        uint32_t r0[32];
-        tmem_ld32(tmem + lane_base + 384 + sub * 32, r0);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive_elect(hacc_empty);  // TMEM H is free: GEMM1(j + 1) may start while this chunk is in the GELU below
-        // ptxas hoists the (register-only) GELU arithmetic above the arrive unless something the arithmetic needs is ordered
-        // after it: the bias slice is loaded behind a CTA fence, which loads cannot cross (v1 / v3 profiles: the release came
-        // ~300 instructions late and GEMM1(j + 1) waited for GELU(j)).
-        __threadfence_block();
-        const float* bias = args.b1 + j * HC + sub * 32;
-        float4 bv[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c)
-          asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];"
-                       : "=f"(bv[c].x), "=f"(bv[c].y), "=f"(bv[c].z), "=f"(bv[c].w)
-                       : "l"(bias + c * 4)
-                       : "memory");
-        uint32_t pk[16];
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          const float4 bb = bv[c >> 2];
-          const float2 g0 = gelu2(make_float2(__uint_as_float(r0[c]) + bb.x, __uint_as_float(r0[c + 1]) + bb.y));
-          const float2 g1 = gelu2(make_float2(__uint_as_float(r0[c + 2]) + bb.z, __uint_as_float(r0[c + 3]) + bb.w));
-          pk[c / 2] = pack_bf16(g0.x, g0.y), pk[c / 2 + 1] = pack_bf16(g1.x, g1.y);
-        }
-        mbar_wait(hs_empty, hs_phase ^ 1);  // GEMM2(j - 1) has finished reading the chunk buffer
-        hs_phase ^= 1;
-        // chunk column c lives in k-block c / 64, 16-byte chunk (c % 64) / 8 at position chunk ^ (row % 8)
-        uint8_t* rowp = sH + (sub >> 1) * 16384 + (r_in_tile >> 3) * 1024 + (r_in_tile & 7) * 128;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int ch = (sub & 1) * 4 + c;
-          *reinterpret_cast<uint4*>(rowp + ((ch ^ (r_in_tile & 7)) << 4)) =
-              make_uint4(pk[c * 4], pk[c * 4 + 1], pk[c * 4 + 2], pk[c * 4 + 3]);
-        }
-        fence_proxy_async_smem();
-        mbar_arrive_elect(hs_full);
-      }
-      // ---- final epilogue: TMEM columns 0..383 already hold x + b2 + FF(LN(x)); 3 chunks of 32 columns per warp
-      mbar_wait(y_full, tphase);
-      tc_fence_after();
+        // ---- GEMM1(j): this warpgroup's 64 hidden columns, K = 384: 6 k-blocks x 4 k-steps of m64n64k16
+        float h[32];
+        int prev1 = -1;
 #pragma unroll 1
-      for (int chunk = sub; chunk < D / 32; chunk += 4) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(tmem + lane_base + chunk * 32, r);
-        tmem_ld_wait();
-        if (lane == 0) tma_store_wait_read<0>();
-        __syncwarp();
+        for (int kb = 0; kb < D / 64; ++kb) {
+          mbar_wait(&w1_full[s1], ph1);
+          const uint64_t ad = wgmma_desc_sw128(smem_u32(sA + kb * 8192));
+          const uint64_t bd = wgmma_desc_sw128(smem_u32(sW1 + s1 * kS1Bytes + g * 8192));
+          wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 32; c += 8)
-          *reinterpret_cast<uint4*>(my_store + lane * 64 + c * 2) =
-              make_uint4(pack_bf16(__uint_as_float(r[c]), __uint_as_float(r[c + 1])),
-                         pack_bf16(__uint_as_float(r[c + 2]), __uint_as_float(r[c + 3])),
-                         pack_bf16(__uint_as_float(r[c + 4]), __uint_as_float(r[c + 5])),
-                         pack_bf16(__uint_as_float(r[c + 6]), __uint_as_float(r[c + 7])));
+          for (int k = 0; k < 4; ++k) wgmma_ss<0, 0>(h, ad + 2 * k, bd + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();  // everything before this k-block is complete: GEMM2(j - 1) (kb == 0) or k-block kb - 1
+          if (lane == 0) {
+            if (kb == 0 && j > 0) {  // the two W2 slots of GEMM2(j - 1)
+              release(&w2_empty[s2]);
+              release(&w2_empty[s2 ^ 1]);
+            }
+            if (prev1 >= 0) release(&w1_empty[prev1]);
+          }
+          prev1 = s1;
+          if (++s1 == kS1) s1 = 0, ph1 ^= 1;
+        }
+        wgmma_wait<0>();
+        if (lane == 0) release(&w1_empty[prev1]);
+        // ---- + b1, GELU, bf16 -> chunk buffer j % 2 (k-block g: its 64 columns are this warpgroup's)
+        uint8_t* hb = sH + (j & 1) * kHBytes + g * 8192;
+#pragma unroll
+        for (int jj = 0; jj < 8; jj += 2) {
+          float v[8];
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(args.b1 + j * HC + g * 64 + (jj + u) * 8 + quad * 2));
+            v[4 * u + 0] = h[(jj + u) * 4 + 0] + b.x, v[4 * u + 1] = h[(jj + u) * 4 + 1] + b.y;
+            v[4 * u + 2] = h[(jj + u) * 4 + 2] + b.x, v[4 * u + 3] = h[(jj + u) * 4 + 3] + b.y;
+          }
+          gelu_erf8(v);
+#pragma unroll
+          for (int u = 0; u < 2; ++u)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int r = r0 + hh * 8;
+              // column 8 (jj + u) + 2 quad of the k-block: 16-byte chunk jj + u at position chunk ^ (row % 8)
+              *reinterpret_cast<uint32_t*>(hb + (r >> 3) * 1024 + (r & 7) * 128 + (((jj + u) ^ (r & 7)) << 4) + quad * 4) =
+                  pack_bf16(v[4 * u + 2 * hh], v[4 * u + 2 * hh + 1]);
+            }
+        }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmOut, my_store, chunk * 32, tm * BM + quarter * 32);
-          tma_store_commit();
+        // The other warpgroup passed this barrier for chunk j - 1 only after its GEMM2(j - 2) had completed, so buffer
+        // j % 2 was free when it was written above; now both halves of chunk j are visible.
+        consumer_barrier();
+        // ---- GEMM2(j): y[:, 192 g ..] += GELU(H_j) · W2[192 g .., chunk]^T, K = 128: 2 k-blocks x 4 k-steps of m64n192k16
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < HC / 64; ++kb) {
+          mbar_wait(&w2_full[s2], ph2);
+          const uint64_t ad = wgmma_desc_sw128(smem_u32(sH + (j & 1) * kHBytes + kb * 8192));
+          const uint64_t bd = wgmma_desc_sw128(smem_u32(sW2 + s2 * kS2Bytes + g * (kS2Bytes / 2)));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_ss<0, 0>(y, ad + 2 * k, bd + 2 * k, (j | kb | k) != 0 ? 1u : 0u);
+          if (++s2 == kS2) s2 = 0, ph2 ^= 1;
+        }
+        wgmma_commit();
+      }
+      wgmma_wait<0>();
+      if (lane == 0) {
+        release(&w2_empty[s2]);
+        release(&w2_empty[s2 ^ 1]);
+      }
+      // ---- epilogue: out = y + x + b2
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const long row = (long)tm * BM + r0 + hh * 8;
+        if (row >= args.M) continue;
+        const bf16* xr = args.x + row * args.ldx + g * 192 + quad * 2;
+        bf16* orow = args.out + row * args.ldo + g * 192 + quad * 2;
+#pragma unroll
+        for (int jj = 0; jj < 24; ++jj) {
+          const uint32_t xv = __ldg(reinterpret_cast<const uint32_t*>(xr + jj * 8));
+          const float2 b = __ldg(reinterpret_cast<const float2*>(args.b2 + g * 192 + jj * 8 + quad * 2));
+          *reinterpret_cast<uint32_t*>(orow + jj * 8) =
+              pack_bf16(y[jj * 4 + 2 * hh] + bf16_lo(xv) + b.x, y[jj * 4 + 2 * hh + 1] + bf16_hi(xv) + b.y);
         }
       }
-      tc_fence_before();
-      if (lane == 0) tma_store_wait_read<0>();  // the staging area is the next tile's H buffer
-      __syncwarp();
-      tphase ^= 1;
     }
-    if (lane == 0) tma_store_wait<0>();
-    __syncwarp();
   }
-
-  tc_fence_before();
-  if (CM > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
-  }
+  // no CTA may retire while a peer can still multicast into it or arrive on its barriers
+  if (CM > 1) cluster_sync_all();
 }
 
-int ff_uniform_issue() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("N1_FF_UI");
-    v = e ? atoi(e) : 1;   // validated: tests/test_ops_gpu.py::test_ff_block with N1_FF_UI=1, 7 % faster (profiles/)
-  }
-  return v;
-}
-
-template <int CM, bool UI>
-void launch_ff(const bf16* w1, const bf16* w2, const FfArgs& a, bf16* out, int ldo, cudaStream_t stream) {
+template <int CM>
+void launch_ff(const bf16* w1, const bf16* w2, const FfArgs& a, cudaStream_t stream) {
   static std::once_flag once;
   static int max_clusters = 0;
   std::call_once(once, [] {
-    cudaFuncSetAttribute(ff_block_kernel<CM, UI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    cudaFuncSetAttribute(ff_block_kernel<CM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     max_clusters = device_sm_count() / CM;
     if (CM > 1) {
       cudaLaunchConfig_t cfg = {};
@@ -470,12 +312,11 @@ void launch_ff(const bf16* w1, const bf16* w2, const FfArgs& a, bf16* out, int l
       at.val.clusterDim.x = CM, at.val.clusterDim.y = 1, at.val.clusterDim.z = 1;
       cfg.attrs = &at, cfg.numAttrs = 1;
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, ff_block_kernel<CM, UI>, &cfg) == cudaSuccess && n > 0) max_clusters = n;
+      if (cudaOccupancyMaxActiveClusters(&n, ff_block_kernel<CM>, &cfg) == cudaSuccess && n > 0) max_clusters = n;
     }
   });
   CUtensorMap tmW1 = tma_map_2d(w1, F, D, D, HC / CM, 64, true);
-  CUtensorMap tmW2 = tma_map_2d(w2, D, F, F, 192 / CM, 64, true);
-  CUtensorMap tmOut = tma_map_2d(out, a.M, D, ldo, 32, 32, false);
+  CUtensorMap tmW2 = tma_map_2d(w2, D, F, F, 192, 64, true);
   const int super_m = (a.tiles_m + CM - 1) / CM;
   const int clusters = super_m < max_clusters ? super_m : max_clusters;
   cudaLaunchConfig_t cfg = {};
@@ -485,7 +326,7 @@ void launch_ff(const bf16* w1, const bf16* w2, const FfArgs& a, bf16* out, int l
   at.val.clusterDim.x = CM, at.val.clusterDim.y = 1, at.val.clusterDim.z = 1;
   cfg.attrs = &at, cfg.numAttrs = 1;
   const int ticket = prof_begin(4.0 * a.M * (double)D * F, a.M, -F, D, stream);  // N = -1536 marks the fused FF block
-  N1_CUDA(cudaLaunchKernelEx(&cfg, ff_block_kernel<CM, UI>, tmW1, tmW2, tmOut, a));
+  N1_CUDA(cudaLaunchKernelEx(&cfg, ff_block_kernel<CM>, tmW1, tmW2, a));
   prof_end(ticket, stream);
   prof_count_gemm(4.0 * a.M * (double)D * F);
   N1_CUDA(cudaGetLastError());
@@ -500,15 +341,12 @@ void ff_block_384(const bf16* x, int ldx, const float* ln_w, const float* ln_b, 
   if (M <= 0) return;
   N1_CHECK(x && out && w1 && w2 && ln_w && ln_b && b1 && b2, "ff_block_384: null pointer");
   N1_CHECK((reinterpret_cast<uintptr_t>(x) & 15) == 0 && ldx % 8 == 0, "ff_block_384: misaligned x");
+  N1_CHECK((reinterpret_cast<uintptr_t>(out) & 3) == 0 && ldo % 2 == 0, "ff_block_384: misaligned out");
   FfArgs a;
   a.M = M, a.tiles_m = (M + BM - 1) / BM;
-  a.x = x, a.ldx = ldx, a.ln_w = ln_w, a.ln_b = ln_b, a.eps = eps, a.b1 = b1, a.b2 = b2;
-  const bool ui = ff_uniform_issue() != 0;
-  if (cluster >= 2 && a.tiles_m >= 2) {
-    if (ui) launch_ff<2, true>(w1, w2, a, out, ldo, stream); else launch_ff<2, false>(w1, w2, a, out, ldo, stream);
-  } else {
-    if (ui) launch_ff<1, true>(w1, w2, a, out, ldo, stream); else launch_ff<1, false>(w1, w2, a, out, ldo, stream);
-  }
+  a.x = x, a.ldx = ldx, a.ln_w = ln_w, a.ln_b = ln_b, a.eps = eps, a.b1 = b1, a.b2 = b2, a.out = out, a.ldo = ldo;
+  if (cluster >= 2 && a.tiles_m >= 2) launch_ff<2>(w1, w2, a, stream);
+  else launch_ff<1>(w1, w2, a, stream);
 }
 
 }  // namespace n1

@@ -1,0 +1,480 @@
+// Persistent warp-specialised bf16 GEMM for sm_90a:  out = epilogue(A[M,K] @ W[N,K]^T).
+//
+//   warpgroups 0-1  consumers: each owns 64 of the tile's 128 rows: wgmma m64nBNk16 from shared memory into fp32
+//                   register accumulators (one k-block in flight while the previous one's slot is released), then the
+//                   epilogue straight from the accumulator fragments: bias / activation / layer-scale / residual, bf16
+//                   tiles through a per-warp staging buffer and TMA stores (or direct stores for fp32 / remapped rows).
+//   warp 8          producer: one thread issues the TMA loads (cp.async.bulk.tensor 2-D, 128-byte swizzle) into a
+//                   STAGES-deep mbarrier ring.
+// Tiles are 128 x 128 or 128 x 64: with three warps on one scheduler ptxas allots 168 registers per thread, which the 128
+// accumulators of a 128 x 256 tile plus the epilogue exceed (it spilled).
+//
+// This one kernel carries every Linear / Conv-as-GEMM on the InternVLA-N1 hot path (SURVEY.md §2.1):
+// the reference reaches cuBLAS through nn.Linear at navdp.py L57-66/L94-100, navdp_backbone.py L147-149,
+// dinov2_layers/{attention.py L46-48, mlp.py L30-32, patch_embed.py L65} and the Qwen2.5-VL blocks.
+#include <stdlib.h>
+
+#include <algorithm>
+#include <atomic>
+#include <mutex>
+#include <vector>
+
+#include "n1_ops.h"
+#include "n1_ptx.cuh"
+
+namespace n1 {
+
+namespace {
+
+constexpr int BM = 128;
+constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle row
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * kConsumerWarps + 32;
+
+template <int BN>
+struct Cfg {
+  static constexpr int kABytes = BM * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kStages = BN >= 128 ? 6 : 8;
+  static constexpr int kBarBytes = 256;
+  static constexpr int kStoreBytes = kConsumerWarps * 2 * 1024;  // per-warp double-buffered 16x32 bf16 staging for TMA stores
+  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + kStoreBytes + 1024;  // +1024: manual alignment
+};
+static_assert(Cfg<128>::kSmemBytes <= 232448, "GEMM shared memory budget (227 KB per block)");
+
+struct GemmArgs {
+  int M, N, K;
+  int tiles_m, tiles_n;
+  void* out;
+  int ldo;
+  const float* bias;
+  const float* gamma;
+  const bf16* residual;
+  int ldr;
+  int act;
+  int out_fp32;
+  int rows_per_group, group_stride, group_offset;
+  const float* row_add;
+  int raster_g;   // M tiles per raster group (decode_tile)
+  int tma_store;  // bf16 output tile goes registers -> smem staging -> cp.async.bulk.tensor store (full-sector writes)
+};
+
+// Grouped rasterisation: consecutive tile ids walk G M-tiles before moving to the next N-tile, so the CTAs resident at
+// one time share few W panels, and the A panels of a group stay L2-resident while the group sweeps all N tiles.  DRAM
+// traffic ~ W bytes x (tiles_m / G) + A bytes, so G grows until the group's A panels fill the L2 share given to them.
+__device__ __forceinline__ void decode_tile(int tile, int tiles_m, int tiles_n, int G, int& tm, int& tn) {
+  const int per_group = G * tiles_n;
+  const int g = tile / per_group;
+  const int first_m = g * G;
+  const int gsize = min(G, tiles_m - first_m);
+  const int r = tile - g * per_group;
+  tm = first_m + r % gsize;
+  tn = r / gsize;
+}
+
+__device__ __forceinline__ float apply_act(float v, int act) {
+  if (act == ACT_GELU) return gelu_erf(v);
+  if (act == ACT_RELU) return fmaxf(v, 0.0f);
+  if (act == ACT_GELU_TANH)  // nn.GELU(approximate="tanh"): the NextDiT condition projections
+    return 0.5f * v * (1.0f + tanhf(0.7978845608028654f * (v + 0.044715f * v * v * v)));
+  if (act == ACT_SILU) return silu(v);
+  return v;
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const GemmArgs args) {
+  using C = Cfg<BN>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + C::kStages * C::kABytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + C::kStages;
+  uint8_t* sStore = smem + C::kStages * C::kStageBytes + C::kBarBytes;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_tiles = args.tiles_m * args.tiles_n;
+  const int nkb = (args.K + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    if (args.tma_store) tma_prefetch_desc(&tmC);
+    for (int s = 0; s < C::kStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], kConsumerWarps);  // every consumer warp releases the slot once its own MMAs have read it
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    // ------------------------------------------------------------------ TMA producer
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int tm, tn;
+        decode_tile(tile, args.tiles_m, args.tiles_n, args.raster_g, tm, tn);
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&full[stage], C::kStageBytes);
+          tma_load_2d(sA + stage * C::kABytes, &tmA, &full[stage], kb * BK, tm * BM);
+          tma_load_2d(sB + stage * C::kBBytes, &tmB, &full[stage], kb * BK, tn * BN);
+          if (++stage == C::kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+  } else {
+    // ------------------------------------------------------------------ consumers: main loop + epilogue
+    const int wg = warp >> 2;               // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int wrow = wg * 64 + (warp & 3) * 16;  // first of this warp's 16 rows
+    const int quad = lane & 3;
+    const bool swiglu = args.act == ACT_SWIGLU;
+    uint8_t* my_store = sStore + warp * 2048;
+    int sbuf = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int tm, tn;
+      decode_tile(tile, args.tiles_m, args.tiles_n, args.raster_g, tm, tn);
+      float acc[BN / 2];
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint64_t adesc = wgmma_desc_sw128(smem_u32(sA + stage * C::kABytes + wg * 64 * 128));
+        const uint64_t bdesc = wgmma_desc_sw128(smem_u32(sB + stage * C::kBBytes));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)  // 16 elements (32 bytes) along K inside the swizzle row: +2 in 16-byte units
+          wgmma_ss<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have read their slot
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == C::kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+      // ---- epilogue: this thread holds rows r[0], r[1] = r[0] + 8 and, per 8-column group, 2 adjacent columns
+      int row[2];
+      long out_row[2];
+      int grp_row[2] = {0, 0};
+      bool row_ok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        row[h] = tm * BM + wrow + (lane >> 2) + h * 8;
+        row_ok[h] = row[h] < args.M;
+        out_row[h] = row[h];
+        if (args.rows_per_group > 0) {
+          grp_row[h] = row[h] % args.rows_per_group;
+          out_row[h] = (long)(row[h] / args.rows_per_group) * args.group_stride + grp_row[h] + args.group_offset;
+        }
+      }
+#pragma unroll
+      for (int chunk = 0; chunk < BN / 32; ++chunk) {  // unrolled: the accumulator is indexed statically
+        const int col0 = tn * BN + chunk * 32;
+        if (col0 >= args.N) break;  // block-uniform
+        float v[4][4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int col = col0 + j * 8 + quad * 2;
+          const bool col_ok = col < args.N;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) v[j][e] = acc[(chunk * 4 + j) * 4 + e];
+          if (args.bias && col_ok) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(args.bias + col));
+            v[j][0] += b.x, v[j][1] += b.y, v[j][2] += b.x, v[j][3] += b.y;
+          }
+          if (swiglu) {  // (gate, up) interleaved: this thread's column pair -> one output
+            v[j][0] = silu(v[j][0]) * v[j][1];
+            v[j][2] = silu(v[j][2]) * v[j][3];
+            continue;
+          }
+#pragma unroll
+          for (int e = 0; e < 4; ++e) v[j][e] = apply_act(v[j][e], args.act);
+          if (args.gamma && col_ok) {
+            const float2 g = __ldg(reinterpret_cast<const float2*>(args.gamma + col));
+            v[j][0] *= g.x, v[j][1] *= g.y, v[j][2] *= g.x, v[j][3] *= g.y;
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!row_ok[h] || !col_ok) continue;
+            if (args.row_add) {
+              const float2 a = __ldg(reinterpret_cast<const float2*>(args.row_add + (long)grp_row[h] * args.N + col));
+              v[j][2 * h] += a.x, v[j][2 * h + 1] += a.y;
+            }
+            if (args.residual) {
+              const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(args.residual + out_row[h] * args.ldr + col));
+              v[j][2 * h] += bf16_lo(q), v[j][2 * h + 1] += bf16_hi(q);
+            }
+          }
+        }
+        if (args.tma_store) {
+          // 16 rows x 32 columns (SwiGLU: 16 output columns) staged per warp, then one bulk tensor store
+          if (lane == 0) tma_store_wait_read<1>();
+          __syncwarp();
+          uint8_t* sb = my_store + sbuf * 1024;
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = (lane >> 2) + h * 8;
+              if (swiglu)
+                *reinterpret_cast<bf16*>(sb + r * 32 + (j * 4 + quad) * 2) = __float2bfloat16_rn(v[j][2 * h]);
+              else
+                *reinterpret_cast<uint32_t*>(sb + r * 64 + (j * 8 + quad * 2) * 2) = pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
+            }
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (lane == 0) {
+            // rows >= M / cols >= N are clipped by the tensor map
+            tma_store_2d(&tmC, sb, swiglu ? col0 >> 1 : col0, tm * BM + wrow);
+            tma_store_commit();
+          }
+          sbuf ^= 1;
+          continue;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int col = col0 + j * 8 + quad * 2;
+          if (col >= args.N) continue;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!row_ok[h]) continue;
+            if (swiglu)
+              reinterpret_cast<bf16*>(args.out)[out_row[h] * args.ldo + (col >> 1)] = __float2bfloat16_rn(v[j][2 * h]);
+            else if (args.out_fp32)
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(args.out) + out_row[h] * args.ldo + col) =
+                  make_float2(v[j][2 * h], v[j][2 * h + 1]);
+            else
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(args.out) + out_row[h] * args.ldo + col) =
+                  pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
+          }
+        }
+      }
+    }
+    if (args.tma_store && lane == 0) tma_store_wait<0>();
+    __syncwarp();
+  }
+}
+
+// ------------------------------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
+    if (e == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  if (!fn) throw Error(-4, "cuTensorMapEncodeTiled unavailable (no CUDA driver / GPU?)");
+  return fn;
+}
+
+// 2-D bf16 tensor map over a row-major [rows, cols] matrix with leading dimension ld; box = [box_rows, box_cols];
+// operands use box_cols = 64 with the 128-byte swizzle, output staging tiles are unswizzled.
+CUtensorMap make_map(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols = BK, bool swizzle = true) {
+  N1_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "GEMM operand not 16-byte aligned");
+  N1_CHECK(ld % 8 == 0, "GEMM operand leading dimension must be a multiple of 8 elements");
+  CUtensorMap m;
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<bf16*>(ptr), gdim, gstr, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) throw Error(-5, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
+  return m;
+}
+
+template <int BN>
+void launch(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, GemmArgs& a, cudaStream_t stream) {
+  using C = Cfg<BN>;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    cudaFuncSetAttribute(gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+  });
+  a.tiles_m = (M + BM - 1) / BM;
+  a.tiles_n = (N + BN - 1) / BN;
+  {
+    // raster group: as many M tiles of A as fit a third of the 50 MB L2 (W streams through the rest); only matters
+    // when W does not fit L2
+    const long panel = (long)BM * K * 2;
+    const long w_bytes = (long)N * K * 2;
+    int g = 8;
+    if (w_bytes > (32L << 20)) g = (int)std::max<long>(2, (16L << 20) / panel);
+    a.raster_g = g < a.tiles_m ? g : a.tiles_m;
+    if (a.raster_g < 1) a.raster_g = 1;
+  }
+  CUtensorMap tmA = make_map(A, M, K, lda, BM);
+  CUtensorMap tmB = make_map(W, N, K, ldw, BN);
+  CUtensorMap tmC = tmA;  // placeholder when the direct-store epilogue is used
+  if (a.tma_store) {
+    const bool sw = a.act == ACT_SWIGLU;
+    tmC = make_map(static_cast<const bf16*>(a.out), M, sw ? N / 2 : N, a.ldo, 16, sw ? 16 : 32, false);
+  }
+  const int tiles = a.tiles_m * a.tiles_n;
+  const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
+  gemm_kernel<BN><<<grid, kThreads, C::kSmemBytes, stream>>>(tmA, tmB, tmC, a);
+  N1_CUDA(cudaGetLastError());
+}
+
+// ---- profiling state
+std::atomic<long> g_total_launches{0}, g_gemm_launches{0};
+std::atomic<bool> g_prof_on{false};
+std::mutex g_prof_mu;
+struct EvPair {
+  cudaEvent_t a, b;
+  double flops;
+  int M, N, K;
+};
+std::vector<EvPair> g_events;
+struct ShapeAcc {
+  int M, N, K;
+  long count;
+  double ms;
+};
+std::vector<ShapeAcc> g_shapes;  // per-(M, N, K) sums of the event-timed launches since the last prof_read_shapes()
+
+}  // namespace
+
+CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle) {
+  return make_map(ptr, rows, cols, ld, box_rows, box_cols, swizzle);
+}
+// GEMM-class kernels in other files: counted like gemm_bf16 launches (event timing is only done for gemm_bf16)
+void prof_count_gemm(double flops) {
+  (void)flops;
+  g_gemm_launches++;
+  g_total_launches++;
+}
+
+void prof_enable(bool on) { g_prof_on = on; }
+// Event bracket for GEMM-class kernels launched outside gemm_bf16 (the fused decoder blocks): returns a ticket (< 0: off)
+int prof_begin(double flops, int M, int N, int K, cudaStream_t s) {
+  if (!g_prof_on.load()) return -1;
+  EvPair ev{};
+  cudaEventCreate(&ev.a);
+  cudaEventCreate(&ev.b);
+  ev.flops = flops, ev.M = M, ev.N = N, ev.K = K;
+  cudaEventRecord(ev.a, s);
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  g_events.push_back(ev);
+  return (int)g_events.size() - 1;
+}
+void prof_end(int ticket, cudaStream_t s) {
+  if (ticket < 0) return;
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  if (ticket < (int)g_events.size()) cudaEventRecord(g_events[ticket].b, s);
+}
+void prof_count_launch(int n) { g_total_launches += n; }
+ProfStats prof_read_and_reset() {
+  ProfStats st;
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  for (EvPair& e : g_events) {
+    cudaEventSynchronize(e.b);
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, e.a, e.b) == cudaSuccess) {
+      st.gemm_ms += ms, st.gemm_flops += e.flops;
+      bool hit = false;
+      for (ShapeAcc& sa : g_shapes)
+        if (sa.M == e.M && sa.N == e.N && sa.K == e.K) {
+          sa.count++, sa.ms += ms, hit = true;
+          break;
+        }
+      if (!hit) g_shapes.push_back({e.M, e.N, e.K, 1, (double)ms});
+    }
+    cudaEventDestroy(e.a);
+    cudaEventDestroy(e.b);
+  }
+  g_events.clear();
+  st.gemm_launches = g_gemm_launches.exchange(0);
+  st.total_launches = g_total_launches.exchange(0);
+  return st;
+}
+
+int prof_read_shapes(int* mnk, long* count, double* ms, int cap) {
+  std::lock_guard<std::mutex> lk(g_prof_mu);
+  int n = 0;
+  for (const ShapeAcc& sa : g_shapes) {
+    if (n >= cap) break;
+    mnk[3 * n] = sa.M, mnk[3 * n + 1] = sa.N, mnk[3 * n + 2] = sa.K;
+    count[n] = sa.count, ms[n] = sa.ms;
+    ++n;
+  }
+  g_shapes.clear();
+  return n;
+}
+
+int device_sm_count() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (sms <= 0) sms = 132;
+  }
+  return sms;
+}
+
+void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ldo, int M, int N, int K,
+               const GemmEpilogue& e, cudaStream_t stream) {
+  if (M <= 0 || N <= 0) return;
+  N1_CHECK(K > 0 && K % 8 == 0, "GEMM K must be a positive multiple of 8");
+  N1_CHECK(N % 8 == 0, "GEMM N must be a multiple of 8 (pad the packed weight)");
+  N1_CHECK(!(e.act == ACT_SWIGLU) || N % 16 == 0, "SwiGLU GEMM needs N % 16 == 0");
+  GemmArgs a;
+  a.M = M, a.N = N, a.K = K;
+  a.out = out, a.ldo = ldo;
+  a.bias = e.bias, a.gamma = e.gamma, a.residual = e.residual, a.ldr = e.ldr;
+  a.act = e.act, a.out_fp32 = e.out_fp32;
+  a.rows_per_group = e.rows_per_group, a.group_stride = e.group_stride, a.group_offset = e.group_offset;
+  a.row_add = e.row_add;
+  a.tma_store = (!e.out_fp32 && e.rows_per_group == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && ldo % 8 == 0) ? 1 : 0;
+  // Tile-width choice: fewest waves first, then the widest tile (fewer A re-reads, longer MMA bursts).
+  const int sms = device_sm_count();
+  const int tm = (M + BM - 1) / BM;
+  auto cost = [&](int bn) {
+    const long tiles = (long)tm * ((N + bn - 1) / bn);
+    const long waves = (tiles + sms - 1) / sms;
+    return waves * (bn + 48);  // per-tile time ~ BN plus a fixed prologue/epilogue share
+  };
+  EvPair ev{};
+  const bool prof = g_prof_on.load();
+  if (prof) {
+    cudaEventCreate(&ev.a);
+    cudaEventCreate(&ev.b);
+    ev.flops = 2.0 * M * (double)N * K;
+    ev.M = M, ev.N = N, ev.K = K;
+    cudaEventRecord(ev.a, stream);
+  }
+  g_gemm_launches++;
+  g_total_launches++;
+  if (cost(128) <= cost(64)) launch<128>(A, lda, W, ldw, M, N, K, a, stream);
+  else launch<64>(A, lda, W, ldw, M, N, K, a, stream);
+  if (prof) {
+    cudaEventRecord(ev.b, stream);
+    std::lock_guard<std::mutex> lk(g_prof_mu);
+    g_events.push_back(ev);
+  }
+}
+
+}  // namespace n1

@@ -33,7 +33,7 @@ struct Error : std::runtime_error {
 
 // ------------------------------------------------------------------------------------------- GEMM
 // out[M, N'] = epilogue(A[M,K] @ W[N,K]^T).  A and W are bf16, K-major (row-major with leading
-// dimensions lda / ldw in elements, multiples of 8).  Accumulation in fp32 (TMEM).
+// dimensions lda / ldw in elements, multiples of 8).  Accumulation in fp32 (registers).
 enum GemmAct { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SWIGLU = 3, ACT_GELU_TANH = 4, ACT_SILU = 5 };
 
 struct GemmEpilogue {
@@ -57,7 +57,7 @@ int device_sm_count();
 // 2-D bf16 tensor map over a row-major [rows, cols] matrix (leading dimension ld elements); box = [box_rows, box_cols];
 // operand tiles use box_cols = 64 with the 128-byte swizzle, output staging tiles are unswizzled.
 CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle);
-void prof_count_gemm(double flops);  // launch + FLOP accounting for GEMM-class kernels outside gemm_tcgen05.cu
+void prof_count_gemm(double flops);  // launch + FLOP accounting for GEMM-class kernels outside gemm_wgmma.cu
 
 // Launch accounting (always on) and optional per-GEMM event timing (bench.py's roofline pass).
 struct ProfStats {
@@ -96,16 +96,16 @@ struct AttnParams {
   const int* k_len;      // optional [batch_kv] device: slotted K/V (a KV cache) -- sequence kb occupies rows
   int k_slot;            //   [kb * k_slot, kb * k_slot + k_len[kb]); overrides cu_k / seq_k
   long total_rows;       // optional: rows of the packed q / k / v buffers (var-len self-attention); > 0 lets head_dim 128
-                         //   sequences of <= 320 tokens take the tcgen05 kernel (attention_tc.cu), which needs it for TMA
+                         //   sequences of <= 320 tokens take the wgmma kernel (attention_wgmma.cu), which needs it for TMA
 };
 void attention(const AttnParams& p, cudaStream_t stream);
-// tcgen05 / TMEM / TMA attention for head_dim 128, var-len self-attention with <= 320 keys per sequence (attention_tc.cu)
+// wgmma / TMA attention for head_dim 128, var-len self-attention with <= 320 keys per sequence (attention_wgmma.cu)
 bool attention_tc_supported(const AttnParams& p);
 void attention_tc128(const AttnParams& p, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------- fused decoder blocks
 // FF block of the NavDP decoder layer in one kernel (ff_block.cu): out = x + W2 GELU(W1 LayerNorm(x) + b1) + b2 with the
-// residual stream held in tensor memory.  x / out bf16 [M, ld] (may alias), w1 [1536, 384], w2 [384, 1536] contiguous.
+// hidden activations kept on the SM.  x / out bf16 [M, ld] (may alias), w1 [1536, 384], w2 [384, 1536] contiguous.
 void ff_block_384(const bf16* x, int ldx, const float* ln_w, const float* ln_b, float eps, const bf16* w1, const float* b1,
                   const bf16* w2, const float* b2, bf16* out, int ldo, int M, int cluster, cudaStream_t stream);
 

@@ -32,9 +32,8 @@ void linear(const Lin& L, const bf16* A, int lda, void* out, int ldo, int M, Gem
   gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
 }
 
-// N1_FF_BLOCK: 0 = LayerNorm + FF1 + FF2 as three kernels, 1 / 2 = the FF-block kernel (cluster size).  Default 1:
-// validated on B200 (tests/test_ops_gpu.py::test_ff_block, profiles/r2_ff_block_tests_v0.log) and 6 % faster per
-// dual-system step than the three-kernel form (profiles/r2_bench_dual_system_ffblock_v0.json).
+// N1_FF_BLOCK: 0 = LayerNorm + FF1 + FF2 as three kernels, 1 / 2 = the FF-block kernel (cluster size).  Default 1
+// (tests/test_ops_gpu.py::test_ff_block covers cluster sizes 1 and 2).
 int ff_block_mode() {
   static int mode = -1;
   if (mode < 0) {

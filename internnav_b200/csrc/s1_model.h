@@ -71,7 +71,7 @@ class S1Model {
   size_t ws_rgbd(int B) const;
   void rgbd_encode(void* ws, size_t ws_bytes, const float* rgb, const float* depth, bf16* out, int B,
                    cudaStream_t s) const;
-  // Training branch (s1_train.cu; compiled, not yet validated on a B200): the tokens of the FROZEN RGB ViT for the
+  // Training branch (s1_train.cu): the tokens of the FROZEN RGB ViT for the
   // [goal frame, current frame] pairs, as the Q-former sees them -- final LayerNorm, cls dropped, former_pe added --
   // mem bf16 [B, 2 * frames * 256, D]: only the first frames * 256 rows of every environment are written.
   size_t ws_rgb_tokens(int B) const;

@@ -91,7 +91,7 @@ class S2Model {
                     int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const;
   bool has_lm_head() const { return lm_head_.w != nullptr; }
 
-  // ---- training branch, System-2 half (s2_train.cu; STATUS: compiled, not yet validated on a B200)
+  // ---- training branch, System-2 half (s2_train.cu)
   // The decoder is frozen and causal: the TRAJ rows are a chunk appended to the prompt's K/V cache (exactly the latent
   // pass of llm_generate), and d loss / d latent_queries needs the backward of those n_query rows per sample only
   // (oracle/qwen_backward.py).  Both calls take a GENERATION plan over the prompts (without TRAJ tokens) and the SAME

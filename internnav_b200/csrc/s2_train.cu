@@ -1,6 +1,5 @@
 // Training branch, System-2 half: TRAJ-row forward on the prompt's K/V cache and its backward to latent_queries.
 // Algorithm and parity target: oracle/qwen_backward.py (equal to autograd through the padded-batch forward).
-// STATUS: compiled for sm_100a, not yet run on a B200 (see bwd_kernels.h).
 #include <math.h>
 
 #include <algorithm>

@@ -1,15 +1,13 @@
 // Weight gradients without operand transposes:   dW[No, Ko] (+)= dY[M, No]^T · X[M, Ko]      (bf16 in, fp32 out)
 //
 // The contraction runs over the ROWS of both operands (M = tokens: 6 144 ... 98 304 in the System-1 training step), while
-// the output is a small weight-shaped matrix (No, Ko <= a few thousand).  The first training version transposed dY and X
-// with a kernel (545 launches, 6 % of the step, profiles/r2_launches_ddp_train_v1_summary.txt) to feed the K-major GEMM,
-// which then ran on <= 72 of the 148 SMs (one CTA per output tile).  Here:
-//   * both operands are read in place as MN-major UMMA operands: a TMA box of [64 rows x 64 columns] of the row-major
+// the output is a small weight-shaped matrix (No, Ko <= a few thousand).  Transposing dY and X with a kernel to feed the
+// K-major GEMM costs hundreds of launches per step, and one CTA per output tile leaves most SMs idle.  Here:
+//   * both operands are read in place as MN-major wgmma operands: a TMA box of [64 rows x 64 columns] of the row-major
 //     matrix (128-byte rows, 128-byte swizzle) IS the canonical MN-major layout -- 8 rows form a 1024-byte atom (SBO), the
 //     second 64-wide half of the 128-wide tile lies one box (8 KB, LBO) further; a k-step of 16 rows advances 2 KB
-//     (same layout as V in attention_tc.cu, there validated as the B operand; here also as A: instruction-descriptor
-//     bits 15 and 16);
-//   * the M range is SPLIT over CTAs (grid = output tiles x splits ~ 2 x SM count); partial tiles go to an fp32
+//     (same layout as V in attention_wgmma.cu; here both the A and the B operand are transposed by the instruction);
+//   * the M range is SPLIT over CTAs (grid = output tiles x splits ~ SM count); partial tiles go to an fp32
 //     workspace and a second kernel sums them in a fixed order into the target (deterministic; `accumulate` adds onto
 //     the gradient already in the bucket).
 // Reference: autograd of every nn.Linear of the trainable System-1 branches (navdp.py L291-312 loss.backward()).
@@ -26,7 +24,8 @@ namespace {
 
 constexpr int BM = 128, BN = 128, KB = 64;           // output tile 128 x 128; 64 contraction rows per stage
 constexpr int kStages = 4, kStageBytes = 32768;      // A halves 2 x 8 KB + B halves 2 x 8 KB
-constexpr int kThreads = 192;                        // warp 0 TMA, warp 1 MMA (+ TMEM alloc), warps 2-5 epilogue
+constexpr int kConsumerWarps = 8;                    // two warpgroups, 64 output rows each
+constexpr int kThreads = 32 * kConsumerWarps + 32;   // + warp 8: TMA producer
 constexpr int kSmem = kStages * kStageBytes + 256 + 1024;
 
 struct WgradArgs {
@@ -35,16 +34,6 @@ struct WgradArgs {
   float* partial;                                    // [splits][No][Ko] fp32
 };
 
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmX, const WgradArgs args) {
   extern __shared__ uint8_t smem_raw[];
@@ -52,8 +41,6 @@ wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* full = bars;               // [kStages]
   uint64_t* empty = bars + kStages;    // [kStages]
-  uint64_t* acc_full = bars + 2 * kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x % (args.tiles_n * args.tiles_k), sp = blockIdx.x / (args.tiles_n * args.tiles_k);
@@ -63,22 +50,14 @@ wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__
   const int b1 = min(total_blocks, b0 + args.blocks_per_split);
   const int nblk = max(b1 - b0, 0);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmY), tma_prefetch_desc(&tmX);
-    for (int s = 0; s < kStages; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], 1);
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < kStages; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], kConsumerWarps);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     if (lane == 0) {
       int slot = 0;
       uint32_t ph = 0;
@@ -95,68 +74,42 @@ wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__
         if (++slot == kStages) slot = 0, ph ^= 1;
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0 && nblk > 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM, BN) | (1u << 15) | (1u << 16);   // A and B both MN-major
-      int slot = 0;
-      uint32_t ph = 0;
-      for (int b = 0; b < nblk; ++b) {
-        mbar_wait(&full[slot], ph);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + slot * kStageBytes);
-#pragma unroll
-        for (int ks = 0; ks < KB / 16; ++ks) {
-          const uint64_t ad = desc_mn_sw128(st + ks * 2048, 8192);
-          const uint64_t bd = desc_mn_sw128(st + 16384 + ks * 2048, 8192);
-          umma_f16(tmem, ad, bd, idesc, (b | ks) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty[slot]);
-        if (++slot == kStages) slot = 0, ph ^= 1;
-      }
-      umma_commit(acc_full);
-    }
-    __syncwarp();
   } else {
-    // ------------------------------------------------------------------ epilogue: TMEM -> fp32 partial tile
-    const int quarter = warp & 3;   // TMEM lane quarter of this warp (warp id % 4): warps 2, 3, 4, 5 -> quarters 2, 3, 0, 1
-    const int r = tn * BM + quarter * 32 + lane;
-    float* prow = args.partial + ((size_t)sp * args.No + r) * args.Ko + tk * BN;
-    const bool row_ok = r < args.No;
-    if (nblk > 0) {
-      mbar_wait(acc_full, 0);
-      tc_fence_after();
-    }
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t v[32];
-      if (nblk > 0) {
-        tmem_ld32(tmem + (uint32_t(quarter * 32) << 16) + c, v);
-        tmem_ld_wait();
-      } else {
+    const int wg = warp >> 2;  // output rows [64 wg, 64 wg + 64) of the tile = the wg-th 64-column box of dY
+    float acc[64];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = 0u;   // a split with no rows contributes zeros
-      }
-      if (row_ok) {
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;   // a split with no rows contributes zeros
+    int slot = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int b = 0; b < nblk; ++b) {
+      mbar_wait(&full[slot], ph);
+      const uint32_t st = smem_u32(smem + slot * kStageBytes);
+      wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          const int col = tk * BN + c + i;
-          if (col + 3 < args.Ko) {
-            *reinterpret_cast<float4*>(prow + c + i) = make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]),
-                                                                   __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-          } else {
-            for (int e = 0; e < 4; ++e)
-              if (col + e < args.Ko) prow[c + i + e] = __uint_as_float(v[i + e]);
-          }
-        }
+      for (int ks = 0; ks < KB / 16; ++ks) {
+        const uint64_t ad = wgmma_desc_sw128(st + wg * 8192 + ks * 2048);
+        const uint64_t bd = wgmma_desc_sw128(st + 16384 + ks * 2048, 8192);
+        wgmma_ss<1, 1>(acc, ad, bd, 1u);   // A and B both MN-major
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = slot;
+      if (++slot == kStages) slot = 0, ph ^= 1;
+    }
+    wgmma_wait<0>();
+    // ------------------------------------------------------------------ epilogue: accumulators -> fp32 partial tile
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = tn * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2) + h * 8;
+      if (r >= args.No) continue;
+      float* prow = args.partial + ((size_t)sp * args.No + r) * args.Ko;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = tk * BN + j * 8 + (lane & 3) * 2;   // Ko % 4 == 0: a column pair is inside or outside together
+        if (col < args.Ko) *reinterpret_cast<float2*>(prow + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 128);
   }
 }
 
@@ -174,7 +127,7 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, int split
 int wgrad_tn_splits(int M, int No, int Ko) {
   const int tiles = ((No + BM - 1) / BM) * ((Ko + BN - 1) / BN);
   const int blocks = (M + KB - 1) / KB;
-  int splits = device_sm_count() / tiles;   // one wave of CTAs (132 KB of shared memory each: one CTA per SM)
+  int splits = device_sm_count() / tiles;   // one wave of CTAs (129 KB of shared memory each: one CTA per SM)
   if (splits > blocks) splits = blocks;
   if (splits > 64) splits = 64;
   return splits < 1 ? 1 : splits;

@@ -12,7 +12,7 @@ The reference trains through HF Trainer -> torch DistributedDataParallel with `d
 
 What is different by construction: gradients LIVE in the bucket buffers (`GradientBuckets.grads` are views), so a
 backward kernel writes its result where the collective reads it and nothing is copied or re-flattened per step; each
-bucket is one `all_reduce` on the caller's process group (NCCL over NVLink/NVSwitch on B200s, gloo in the CPU tests),
+bucket is one `all_reduce` on the caller's process group (NCCL over NVLink/NVSwitch on H100s, gloo in the CPU tests),
 issued asynchronously so that the remaining backward overlaps it.
 """
 from collections import OrderedDict

@@ -9,7 +9,7 @@ internvla_n1.py L349-432) for a batch of environments:
          B * Ns trajectories of 32 steps, classifier-free guidance batch [null | cond]
       -> trajectories [B * Ns, 32, 3]
 
-Every matrix product, attention, normalisation and the sampler update run in the library (tcgen05 GEMM, the attention
+Every matrix product, attention, normalisation and the sampler update run in the library (wgmma GEMM, the attention
 kernels, csrc/nextdit_kernels.cu); this module is the schedule -- it orders the launches, owns the packed weights and the
 per-call conditioning tables.  PyTorch is used for buffers and for a handful of per-CALL shape operations on tensors of a
 few kilobytes (concatenating the condition tokens, the 10 x groups modulation inputs); nothing per trajectory row.

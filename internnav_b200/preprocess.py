@@ -9,7 +9,7 @@ The reference prepares every System-1 call on the host, frame by frame, with Pil
 for the remembered goal frame and the current frame.  `FramePreprocessor` does the same for all environments of a step
 in a handful of launches: raw uint8 / float32 frames are copied to the device once and resampled there by
 `n1_resize_rgb_u8` / `n1_resize_f32`, which reproduce Pillow's resampler bit for bit (csrc/resize.cu).  There is no
-host fallback: without the library or a B200 the constructor raises.
+host fallback: without the library or an H100 the constructor raises.
 """
 import ctypes
 from ctypes import c_void_p

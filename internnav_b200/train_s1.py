@@ -2,7 +2,7 @@
 `forward_vlm_traj` + masked MSE (navdp.py L291-312, internvla_n1.py L287-303), as a sequence of kernel calls.
 
 The schedule follows oracle/navdp_backward.py (the backward specification, equal to the reference's autograd) one
-primitive at a time; every matrix product -- forward, dgrad (dY W) and wgrad (dY^T X) -- goes through the tcgen05 GEMM
+primitive at a time; every matrix product -- forward, dgrad (dY W) and wgrad (dY^T X) -- goes through the wgmma GEMM
 (`ops.mm_nt`, operands transposed by a kernel where the contraction runs over rows), attention / LayerNorm / GELU / ReLU /
 layer-scale forward and backward through the kernels of attention.cu, norm.cu and bwd_kernels.cu.  What stays in PyTorch
 is tensor plumbing on bf16 buffers: slicing, concatenation, additions of equally shaped buffers.  The im2col of the
@@ -11,10 +11,10 @@ products too narrow for a tensor-core tile or held in fp32 (the 3-wide action em
 position-table resample and their gradients) go through the library's small fp32 product (`ops.sgemm`).
 
 `ops` is the kernel backend.  The product backend is `GpuOps` below (ctypes -> libn1b200.so; it refuses to run without
-the library / a B200).  tests/test_train_s1_host.py drives this same schedule with a plain fp32 PyTorch implementation of
+the library / an H100).  tests/test_train_s1_host.py drives this same schedule with a plain fp32 PyTorch implementation of
 the `ops` contract on the CPU and checks every gradient against the oracle -- that validates the schedule, not the
-kernels.  The kernels are validated on the B200 by tests/test_bwd_ops_gpu.py (op level, System-2 half, and the whole step
-against the oracle chain; profiles/r2_bwd_ops_parity.log).
+kernels.  The kernels are validated on the H100 by tests/test_bwd_ops_gpu.py (op level, System-2 half, and the whole step
+against the oracle chain).
 """
 import math
 

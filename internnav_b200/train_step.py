@@ -71,7 +71,7 @@ class DualSystemTrainer:
         self.steps, self._micro, self._touched = 0, 0, set()
         self.profile_phases = False
         # graph_s1: replay the System-1 forward / backward (several thousand kernel launches driven from Python, one ctypes
-        # call each: the step is host-bound without it, profiles/README.md) from a CUDA graph captured on the first step of
+        # call each: the step is host-bound without it) from a CUDA graph captured on the first step of
         # a given batch shape
         self.graph_s1, self._s1_graphs = bool(graph_s1), {}
         self._s1_views = OrderedDict((k, g) for k, g in self.buckets.grads.items() if k != "model.latent_queries")

@@ -1,6 +1,6 @@
 """BASELINE ARM of bench.py, not the product and not the parity oracle: the reference algorithm as BATCHED eager PyTorch
 on the GPU -- bf16, every Linear through cuBLAS (F.linear), every attention through F.scaled_dot_product_attention
-(flash / memory-efficient kernels), B environments per call.  This is the "PyTorch-eager on the same B200 at batch 64"
+(flash / memory-efficient kernels), B environments per call.  This is the "PyTorch-eager on the same H100 at batch 64"
 denominator of north_star's >= 10x target and the honest kernel-level comparison for the n1b200 path (VERDICT r1, measurement
 item b): same shapes, same batch, library kernels instead of ours.
 

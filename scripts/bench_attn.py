@@ -1,5 +1,5 @@
 """Decoder-prefill attention at the benchmark shape (64 sequences x 304 tokens, 28 / 4 heads, head_dim 128, causal):
-tcgen05 kernel (attention_tc.cu) vs the mma.sync kernel it replaces, CUDA events, L2 flushed.  One JSON line."""
+wgmma kernel (attention_wgmma.cu) vs the mma.sync kernel it replaces, CUDA events, L2 flushed.  One JSON line."""
 import json
 import os
 import sys
@@ -33,6 +33,6 @@ cu = torch.arange(0, (B + 1) * S, S, dtype=torch.int32, device="cuda")
 t_tc = timed(lambda: L.attention_varlen(q, k, v, Hq, Hkv, hd, cu, S, causal=True))
 t_old = timed(lambda: L.attention(q, k, v, Hq, Hkv, hd, B, 0, 0, cu_q=cu, cu_k=cu, max_seq_q=S, causal=True))
 flops = 4.0 * B * Hq * S * S * hd / 2
-print(json.dumps({"shape": "64 x 304 tokens, 28/4 heads, hd 128, causal", "tcgen05_us": t_tc, "mma_sync_us": t_old,
-                  "speedup": t_old / t_tc, "tcgen05_tflops": flops / (t_tc * 1e-6) / 1e12,
+print(json.dumps({"shape": "64 x 304 tokens, 28/4 heads, hd 128, causal", "wgmma_us": t_tc, "mma_sync_us": t_old,
+                  "speedup": t_old / t_tc, "wgmma_tflops": flops / (t_tc * 1e-6) / 1e12,
                   "causal_gflop": flops / 1e9}))

@@ -1,4 +1,4 @@
-"""Developer microbenchmark: n1 tcgen05 GEMM vs cuBLAS (torch.matmul) on the path's shapes.  Prints TFLOP/s."""
+"""Developer microbenchmark: n1 wgmma GEMM vs cuBLAS (torch.matmul) on the path's shapes.  Prints TFLOP/s."""
 import sys
 
 import torch

@@ -1,12 +1,12 @@
 #!/bin/bash
-# SASS evidence per compilation unit of libn1b200.so: which Blackwell instructions each cubin contains.
-# UTCHMMA = tcgen05.mma, LDTM / STTM = tcgen05.ld / st, UTMALDG / UTMASTG = TMA bulk tensor load / store (.MULTICAST),
-# UTCBAR = tcgen05.commit, SYNCS = mbarrier, HMMA = mma.sync (sm_80-class), FFMA2 / FMUL2 = packed fp32.
+# SASS evidence per compilation unit of libn1b200.so: which Hopper instructions each cubin contains.
+# HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / wait, UTMALDG / UTMASTG = TMA bulk tensor load / store (.MULTICAST),
+# SYNCS = mbarrier, HMMA = mma.sync (sm_80-class).
 cd "$(dirname "$0")/../internnav_b200/_build" || exit 1
-printf "%-22s %8s %6s %6s %8s %8s %10s %7s %7s %6s %6s\n" unit UTCHMMA LDTM STTM UTMALDG UTMASTG MULTICAST UTCBAR SYNCS HMMA FFMA2
+printf "%-22s %8s %10s %8s %8s %10s %7s %6s\n" unit HGMMA WARPGROUP UTMALDG UTMASTG MULTICAST SYNCS HMMA
 for o in *.o; do
   s=$(cuobjdump -sass "$o" 2>/dev/null)
   c() { echo "$s" | grep -c "$1"; }
-  printf "%-22s %8d %6d %6d %8d %8d %10d %7d %7d %6d %6d\n" "${o%.o}" "$(c UTCHMMA)" "$(c LDTM)" "$(c STTM)" "$(c UTMALDG)" \
-    "$(c UTMASTG)" "$(c 'UTMALDG.*MULTICAST')" "$(c UTCBAR)" "$(c SYNCS)" "$(c 'HMMA\.')" "$(c FFMA2)"
+  printf "%-22s %8d %10d %8d %8d %10d %7d %6d\n" "${o%.o}" "$(c HGMMA)" "$(c WARPGROUP)" "$(c UTMALDG)" \
+    "$(c UTMASTG)" "$(c 'UTMALDG.*MULTICAST')" "$(c SYNCS)" "$(c 'HMMA\.')"
 done

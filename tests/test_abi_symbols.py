@@ -19,7 +19,7 @@ def test_every_declared_symbol_is_exported():
 
 
 def test_no_gpu_fails_loudly():
-    """Compute entry points must not fall back to anything when no sm_100 device is usable."""
+    """Compute entry points must not fall back to anything when no sm_90 device is usable."""
     import torch
     from internnav_b200 import _lib
     L = _lib.lib()

@@ -69,7 +69,7 @@ def test_dual_system_step_matches_oracle_chain():
     e, e_eager = _rel(traj, ref), _rel(eager, ref)
     print("dual-system trajectories rel err vs oracle chain", e, "bf16 eager chain", e_eager)
     # end of a two-model chain (tiny random-weight Qwen -> goal token -> 20 sampler steps): the reference-equivalent bf16
-    # run itself is at 2.7e-2 here (measured on B200; ours 3.3e-2), above the per-stage 2e-2 bar, so the binding bar for the
+    # run itself is above the per-stage 2e-2 bar here (smoke() prints both errors), so the binding bar for the
     # chained output is the relative one (<= 2x bf16 eager); the per-stage bars are asserted where the stages are tested
     assert e < 4e-2 and e < 2 * e_eager + 2e-3, (e, e_eager)
     # policy wrapper: same trajectories -> same ids as the batched tail

@@ -8,9 +8,9 @@
         reference agent does (internvla_n1_agent.py L133-208), and reproduce the single-threaded results bit for bit.
 
 Tolerance (SURVEY.md §8d): rel-L2 vs the fp32 oracle <= 2x the bf16-eager error (+ 2e-3 slack) and <= 2e-2 -- except
-that at FULL DEPTH with random weights the reference-equivalent bf16-eager run itself sits at 2.1e-2 (latents) / 2.7e-2
-(vision tower), i.e. above the absolute bar, so there the absolute bar is 3e-2 and the binding requirement is that the
-CUDA path is at least as accurate as bf16 eager (measured on B200: 2.26e-2 vs 2.72e-2, 1.88e-2 vs 2.14e-2)."""
+that at FULL DEPTH with random weights the reference-equivalent bf16-eager run itself can sit above the
+absolute bar, so there the absolute bar is 3e-2 and the binding requirement is that the
+CUDA path is at least as accurate as bf16 eager."""
 import threading
 
 import numpy as np

@@ -74,7 +74,7 @@ def test_training_prefix_extraction():
 
 
 def test_resize_plan_needs_a_device():
-    """Compute entry points fail loudly without a B200 (no host fallback behind the C ABI)."""
+    """Compute entry points fail loudly without an H100 (no host fallback behind the C ABI)."""
     from internnav_b200 import _lib
     from internnav_b200.preprocess import FramePreprocessor, _bind
     if torch.cuda.is_available():

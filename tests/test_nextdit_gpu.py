@@ -89,7 +89,7 @@ def test_batched_vs_oracle_and_eager(env):
         out = m.generate_traj(lat.bfloat16(), img, guidance_scale=scale, num_sample_trajs=Ns, x_init=x0)
         e, ee = _rel(out, t_ref), _rel(t_eag, t_ref)
         print("10-step trajectories, guidance %.1f: rel err" % scale, e, "bf16 eager", ee)
-        assert e < 2e-2 and e < 2 * ee + 2e-3, (scale, e, ee)      # measured on B200: 1.4e-2 vs 0.9e-2 (guidance 1)
+        assert e < 2e-2 and e < 2 * ee + 2e-3, (scale, e, ee)
 
 
 def test_environments_are_independent(env):

@@ -2,7 +2,7 @@
 cross-attention K / V sharing, guidance batch, Euler update) executed on the CPU with every library op replaced by a plain
 PyTorch stand-in that enforces the kernels' operand contracts -- against the oracle and the reference-run fixture.  The same
 idea as tests/test_train_s1_host.py: the schedule is host logic and must be testable without a GPU; the kernels
-themselves are tested against the same stand-ins' arithmetic on the B200 (tests/test_nextdit_gpu.py, test_ops_gpu.py)."""
+themselves are tested against the same stand-ins' arithmetic on the H100 (tests/test_nextdit_gpu.py, test_ops_gpu.py)."""
 import math
 import os
 import types

@@ -228,7 +228,7 @@ def test_ff_block(L, M, cluster):
 @pytest.mark.parametrize("lens,causal", [([304] * 4, True), ([304, 300, 129, 128, 1, 257, 320, 64, 17], True),
                                          ([320, 200, 96], False), ([304] * 64, True)])
 def test_attention_tcgen05_hd128(L, lens, causal):
-    """Decoder-prefill attention on tcgen05 (attention_tc.cu): var-len GQA 28 / 4, head_dim 128, packed q|k|v rows with the
+    """Decoder-prefill attention on wgmma (attention_wgmma.cu): var-len GQA 28 / 4, head_dim 128, packed q|k|v rows with the
     decoder's row stride; against fp32 PyTorch per sequence and against the mma.sync kernel it replaces."""
     torch.manual_seed(len(lens) + sum(lens))
     Hq, Hkv, hd = 28, 4, 128
@@ -237,7 +237,7 @@ def test_attention_tcgen05_hd128(L, lens, causal):
     q, k, v = qkv[:, :Hq * hd], qkv[:, Hq * hd:(Hq + Hkv) * hd], qkv[:, (Hq + Hkv) * hd:]
     cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device="cuda")
     o, used = L.attention_varlen(q, k, v, Hq, Hkv, hd, cu, max(lens), causal=causal)
-    assert used, "the tcgen05 kernel should take this shape"
+    assert used, "the wgmma kernel should take this shape"
     old = L.attention(q, k, v, Hq, Hkv, hd, len(lens), 0, 0, cu_q=cu, cu_k=cu, max_seq_q=max(lens), causal=causal)
     s = 0
     worst = 0.0
