@@ -641,7 +641,7 @@ int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int
     p.heads_q = heads_q, p.heads_kv = heads_kv, p.hd = head_dim, p.batch = batch;
     p.cu_q = p.cu_k = cu_seqlens, p.max_seq_q = max_seq, p.total_rows = total_rows;
     p.kv_div = 1, p.causal = causal, p.scale = scale;
-    if (used_tcgen05) *used_tcgen05 = (head_dim == 128 && attention_tc_supported(p)) ? 1 : 0;
+    if (used_tcgen05) *used_tcgen05 = attention_uses_tc(p) ? 1 : 0;
     attention(p, S(stream));
   });
 }

@@ -405,6 +405,16 @@ void launch_attn(const AttnParams& p, cudaStream_t stream) {
 
 }  // namespace
 
+bool attention_uses_tc(const AttnParams& p) {
+  if (p.hd != 128 || !attention_tc_supported(p)) return false;
+  static int tc = -1;  // N1_ATTN_TC=0 keeps the mma.sync kernel
+  if (tc < 0) {
+    const char* e = getenv("N1_ATTN_TC");
+    tc = e ? atoi(e) : 1;
+  }
+  return tc != 0;
+}
+
 void attention(const AttnParams& p, cudaStream_t stream) {
   if (p.batch <= 0) return;
   N1_CHECK(p.heads_kv > 0 && p.heads_q % p.heads_kv == 0, "attention: heads_q must be a multiple of heads_kv");
@@ -421,16 +431,9 @@ void attention(const AttnParams& p, cudaStream_t stream) {
     else launch_attn_small<4>(p, stream);
     return;
   }
-  if (p.hd == 128 && attention_tc_supported(p)) {
-    static int tc = -1;  // N1_ATTN_TC=0 keeps the mma.sync kernel
-    if (tc < 0) {
-      const char* e = getenv("N1_ATTN_TC");
-      tc = e ? atoi(e) : 1;
-    }
-    if (tc) {
-      attention_tc128(p, stream);
-      return;
-    }
+  if (attention_uses_tc(p)) {
+    attention_tc128(p, stream);
+    return;
   }
   switch (p.hd) {
     case 48: launch_attn<48>(p, stream); break;

@@ -101,6 +101,8 @@ struct AttnParams {
 void attention(const AttnParams& p, cudaStream_t stream);
 // wgmma / TMA attention for head_dim 128, var-len self-attention with <= 320 keys per sequence (attention_wgmma.cu)
 bool attention_tc_supported(const AttnParams& p);
+// whether attention(p) runs the wgmma kernel: supported arguments and not disabled by N1_ATTN_TC=0
+bool attention_uses_tc(const AttnParams& p);
 void attention_tc128(const AttnParams& p, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------- fused decoder blocks
