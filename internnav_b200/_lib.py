@@ -165,6 +165,23 @@ def gemm(a, w, bias=None, gamma=None, residual=None, act=ACT_NONE, out_fp32=Fals
     return out
 
 
+def gemm_tile(a, w, out, bias=None, gamma=None, residual=None, act=ACT_NONE, rows_per_group=0, group_stride=0,
+              group_offset=0, row_add=None, tile_n=0):
+    """gemm() into a caller-owned view `out` (fp32 or bf16, any alignment) with the output row remap / row-add of the
+    patch-embedding GEMMs and a forced tile width (tile_n 64 / 128 / 256; 0 = the dispatcher's choice).  For tests and
+    scripts/bench_tiles.py: n1_test_gemm is exported but is not part of include/n1b200.h."""
+    fn = lib().n1_test_gemm
+    fn.restype = c_int
+    fn.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                   c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
+    vp = lambda t: c_void_p(t.data_ptr()) if t is not None else None
+    check(fn(vp(a), a.stride(0), vp(w), w.stride(0), vp(out), out.stride(0), a.shape[0], w.shape[0], a.shape[1],
+             vp(bias), vp(gamma), vp(residual), residual.stride(0) if residual is not None else 0, act,
+             1 if out.dtype == torch.float32 else 0, rows_per_group, group_stride, group_offset, vp(row_add), tile_n,
+             stream_ptr()))
+    return out
+
+
 def layernorm(x, w, b=None, eps=1e-5, rms=False, out=None):
     assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1
     y = torch.empty(x.shape, device=x.device, dtype=torch.bfloat16) if out is None else out

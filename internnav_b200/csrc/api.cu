@@ -587,6 +587,19 @@ int n1_op_gemm(const void* A, int lda, const void* W, int ldw, void* out, int ld
   });
 }
 
+// Test / bench entry point, deliberately not declared in include/n1b200.h: n1_op_gemm plus the output row remap and
+// row-add of GemmEpilogue and a forced tile width (tile_n: 0 = the dispatcher's choice, else 64 / 128 / 256).
+int n1_test_gemm(const void* A, int lda, const void* W, int ldw, void* out, int ldo, int M, int N, int K, const float* bias,
+                 const float* gamma, const void* residual, int ldr, int act, int out_fp32, int rows_per_group,
+                 int group_stride, int group_offset, const float* row_add, int tile_n, void* stream) {
+  return guard([&] {
+    GemmEpilogue e;
+    e.bias = bias, e.gamma = gamma, e.residual = B16(residual), e.ldr = ldr, e.act = act, e.out_fp32 = out_fp32;
+    e.rows_per_group = rows_per_group, e.group_stride = group_stride, e.group_offset = group_offset, e.row_add = row_add;
+    gemm_bf16(B16(A), lda, B16(W), ldw, out, ldo, M, N, K, e, S(stream), tile_n);
+  });
+}
+
 int n1_op_ff_block(const void* x, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w1, const float* b1,
                    const void* w2, const float* b2, void* out, int ldo, int M, int cluster, void* stream) {
   return guard([&] {

@@ -6,10 +6,13 @@
 // replaces three launches (LayerNorm, FF1+GELU GEMM, FF2+residual GEMM) and the HBM round trips of the [rows, 384]
 // normalised input and the [rows, 1536] hidden.  Per CTA, one 64-row tile at a time (persistent over tiles):
 //
-//   warps 8, 9      producers: warp 8 streams W1 through a 3 x 16 KB ring (one [128 x 64] k-block of a hidden chunk per
-//                   slot), warp 9 streams W2 through a 2 x 48 KB ring (one [384 x 64] k-block per slot).  CM = 2: the two
-//                   CTAs of a cluster work on neighbouring row tiles, fetch half of every slot each and multicast it.
-//   warpgroups 0-1  consumers (320 threads leave them 204 registers each), both on the same 64 rows:
+//   warpgroup 2     producers (warps 10, 11 only hand their registers over and leave): warp 8 streams W1 through a
+//                   3 x 16 KB ring (one [128 x 64] k-block of a hidden chunk per slot), warp 9 streams W2 through a
+//                   2 x 48 KB ring (one [384 x 64] k-block per slot).  CM = 2: the two CTAs of a cluster work on
+//                   neighbouring row tiles, fetch half of every slot each and multicast it.
+//   warpgroups 0-1  consumers, both on the same 64 rows.  The 384-thread kernel is compiled for 168 registers per thread;
+//                   the producer warpgroup gives registers back (40) and the consumers take 232 each (setmaxnreg), and
+//                   ptxas reports 0 bytes of spill for both cluster variants:
 //       prologue    x rows -> LayerNorm -> bf16 A operand in shared memory (128-byte swizzled K-major, 48 KB);
 //       per hidden chunk of 128 columns: warpgroup g computes its 64 columns  H = LN(x) · W1[128 j + 64 g ..]^T  (wgmma
 //                   m64n64k16, fp32 registers), adds b1, GELU, and writes them as bf16 into the swizzled chunk buffer
@@ -35,7 +38,7 @@ constexpr int kS2 = 2, kS2Bytes = D * 64 * 2;        // W2 ring: one k-block [38
 constexpr int kABytes = BM * D * 2;                  // 49152: 6 k-blocks of [64 x 64]
 constexpr int kHBytes = BM * HC * 2;                 // 16384: one GELU(H) chunk, 2 k-blocks of [64 x 64]
 constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 32 * kConsumerWarps + 64;  // 320
+constexpr int kThreads = 32 * kConsumerWarps + 128;  // 384: the producers are a whole warpgroup (setmaxnreg)
 constexpr int kSmem = kABytes + 2 * kHBytes + kS1 * kS1Bytes + kS2 * kS2Bytes + 256 + 1024;
 static_assert(kSmem <= 232448, "ff_block: shared memory budget (227 KB per block)");
 
@@ -88,6 +91,7 @@ ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant_
   if (CM > 1) cluster_sync_all(); else __syncthreads();
 
   if (warp >= kConsumerWarps) {
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == kConsumerWarps && lane == 0) {
       // ------------------------------------------------------------------ TMA producer of W1 (GEMM1's ring)
       int slot = 0;
@@ -126,6 +130,7 @@ ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant_
     }
   } else {
     // ------------------------------------------------------------------ 2 consumer warpgroups
+    setmaxnreg_inc<kConsumerRegs>();
     const int cw = warp;                     // 0..7
     const int g = cw >> 2;                   // warpgroup: hidden columns [64 g, +64) of a chunk, output columns [192 g, +192)
     const int quad = lane & 3;
@@ -205,7 +210,9 @@ ff_block_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant_
       fence_proxy_async_smem();
       consumer_barrier();
 
-      float y[96];
+      // Zeroed although the first MMA overwrites it: the accumulator is an in-out operand of every wgmma, and without a
+      // definition here it would count as live through the LayerNorm prologue above (96 registers, which then spills).
+      float y[96] = {};
       for (int j = 0; j < NCH; ++j) {
         // ---- GEMM1(j): this warpgroup's 64 hidden columns, K = 384: 6 k-blocks x 4 k-steps of m64n64k16
         float h[32];

@@ -4,10 +4,11 @@
 //                   register accumulators (one k-block in flight while the previous one's slot is released), then the
 //                   epilogue straight from the accumulator fragments: bias / activation / layer-scale / residual, bf16
 //                   tiles through a per-warp staging buffer and TMA stores (or direct stores for fp32 / remapped rows).
-//   warp 8          producer: one thread issues the TMA loads (cp.async.bulk.tensor 2-D, 128-byte swizzle) into a
-//                   STAGES-deep mbarrier ring.
-// Tiles are 128 x 128 or 128 x 64: with three warps on one scheduler ptxas allots 168 registers per thread, which the 128
-// accumulators of a 128 x 256 tile plus the epilogue exceed (it spilled).
+//   warpgroup 2     producer: one thread of warp 8 issues the TMA loads (cp.async.bulk.tensor 2-D, 128-byte swizzle)
+//                   into a STAGES-deep mbarrier ring; warps 9-11 only hand their registers over and leave.
+// Tiles are 128 x 256, 128 x 128 or 128 x 64.  384 threads put three warps on every scheduler, so the kernel is compiled
+// for 168 registers per thread; after the barrier set-up the producer warpgroup shrinks to 40 and the consumers grow to
+// 232 (setmaxnreg), which holds the 128 accumulators of the 256-wide tile plus the epilogue without spilling.
 //
 // This one kernel carries every Linear / Conv-as-GEMM on the InternVLA-N1 hot path (SURVEY.md §2.1):
 // the reference reaches cuBLAS through nn.Linear at navdp.py L57-66/L94-100, navdp_backbone.py L147-149,
@@ -29,19 +30,22 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle row
 constexpr int kConsumerWarps = 8;
-constexpr int kThreads = 32 * kConsumerWarps + 32;
+constexpr int kThreads = 32 * kConsumerWarps + 128;  // + the producer warpgroup
 
 template <int BN>
 struct Cfg {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = BN >= 128 ? 6 : 8;
+  static constexpr int kStages = BN == 256 ? 4 : BN == 128 ? 6 : 8;
   static constexpr int kBarBytes = 256;
   static constexpr int kStoreBytes = kConsumerWarps * 2 * 1024;  // per-warp double-buffered 16x32 bf16 staging for TMA stores
   static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + kStoreBytes + 1024;  // +1024: manual alignment
 };
-static_assert(Cfg<128>::kSmemBytes <= 232448, "GEMM shared memory budget (227 KB per block)");
+static_assert(Cfg<256>::kSmemBytes <= 232448 && Cfg<128>::kSmemBytes <= 232448 && Cfg<64>::kSmemBytes <= 232448,
+              "GEMM shared memory budget (227 KB per block)");
+
+constexpr long kWStreamsBytes = 32L << 20;  // a W larger than this streams through the 50 MB L2 instead of living in it
 
 struct GemmArgs {
   int M, N, K;
@@ -113,9 +117,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
   __syncthreads();
 
-  if (warp == kConsumerWarps) {
+  if (warp >= kConsumerWarps) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -135,6 +140,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
   } else {
     // ------------------------------------------------------------------ consumers: main loop + epilogue
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;               // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
     const int wrow = wg * 64 + (warp & 3) * 16;  // first of this warp's 16 rows
     const int quad = lane & 3;
@@ -317,11 +323,13 @@ void launch(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K,
   a.tiles_n = (N + BN - 1) / BN;
   {
     // raster group: as many M tiles of A as fit a third of the 50 MB L2 (W streams through the rest); only matters
-    // when W does not fit L2
+    // when W does not fit L2.  The SMs hold sms / G W panels at a time: at K = 3584 (G = 18) that is 7 panels, 6.4 MB
+    // with the 128-wide tile and 12.8 MB with the 256-wide one, which still leaves the rest of the L2 to the stream,
+    // so G does not depend on BN.
     const long panel = (long)BM * K * 2;
     const long w_bytes = (long)N * K * 2;
     int g = 8;
-    if (w_bytes > (32L << 20)) g = (int)std::max<long>(2, (16L << 20) / panel);
+    if (w_bytes > kWStreamsBytes) g = (int)std::max<long>(2, (16L << 20) / panel);
     a.raster_g = g < a.tiles_m ? g : a.tiles_m;
     if (a.raster_g < 1) a.raster_g = 1;
   }
@@ -436,8 +444,9 @@ int device_sm_count() {
 }
 
 void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ldo, int M, int N, int K,
-               const GemmEpilogue& e, cudaStream_t stream) {
+               const GemmEpilogue& e, cudaStream_t stream, int tile_n) {
   if (M <= 0 || N <= 0) return;
+  N1_CHECK(tile_n == 0 || tile_n == 64 || tile_n == 128 || tile_n == 256, "GEMM tile width must be 0, 64, 128 or 256");
   N1_CHECK(K > 0 && K % 8 == 0, "GEMM K must be a positive multiple of 8");
   N1_CHECK(N % 8 == 0, "GEMM N must be a multiple of 8 (pad the packed weight)");
   N1_CHECK(!(e.act == ACT_SWIGLU) || N % 16 == 0, "SwiGLU GEMM needs N % 16 == 0");
@@ -449,14 +458,23 @@ void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ld
   a.rows_per_group = e.rows_per_group, a.group_stride = e.group_stride, a.group_offset = e.group_offset;
   a.row_add = e.row_add;
   a.tma_store = (!e.out_fp32 && e.rows_per_group == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && ldo % 8 == 0) ? 1 : 0;
-  // Tile-width choice: fewest waves first, then the widest tile (fewer A re-reads, longer MMA bursts).
+  // Tile-width choice from the shape and the SM count: the least waves x (BN + fixed prologue / epilogue share), ties to
+  // the wider tile (fewer A re-reads, longer MMA bursts).  The 256-wide tile is a candidate only when W does not fit the
+  // L2 (the raster rule's test in launch()): there the 128-wide tile is held back by operand traffic and 256 wins (LLM
+  // gate/up and down projections, DESIGN.md §5); where W is L2-resident its longer epilogue, during which the tensor
+  // cores idle, costs more than it saves.  tile_n != 0 (tests and scripts/bench_tiles.py) overrides the choice.
   const int sms = device_sm_count();
   const int tm = (M + BM - 1) / BM;
   auto cost = [&](int bn) {
     const long tiles = (long)tm * ((N + bn - 1) / bn);
     const long waves = (tiles + sms - 1) / sms;
-    return waves * (bn + 48);  // per-tile time ~ BN plus a fixed prologue/epilogue share
+    return waves * (bn + 48);
   };
+  int bn = tile_n;
+  if (bn == 0) {
+    bn = cost(128) <= cost(64) ? 128 : 64;
+    if ((long)N * K * 2 > kWStreamsBytes && cost(256) <= cost(bn)) bn = 256;
+  }
   EvPair ev{};
   const bool prof = g_prof_on.load();
   if (prof) {
@@ -468,7 +486,8 @@ void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ld
   }
   g_gemm_launches++;
   g_total_launches++;
-  if (cost(128) <= cost(64)) launch<128>(A, lda, W, ldw, M, N, K, a, stream);
+  if (bn == 256) launch<256>(A, lda, W, ldw, M, N, K, a, stream);
+  else if (bn == 128) launch<128>(A, lda, W, ldw, M, N, K, a, stream);
   else launch<64>(A, lda, W, ldw, M, N, K, a, stream);
   if (prof) {
     cudaEventRecord(ev.b, stream);

@@ -49,8 +49,10 @@ struct GemmEpilogue {
   const float* row_add = nullptr;   // [rows_per_group, N] fp32 added per (row % rows_per_group) (pos-embed)
 };
 
+// tile_n: 0 lets the dispatcher choose the tile width from M, N and the SM count (every model call); 64 / 128 / 256
+// force it (tests and scripts/bench_tiles.py only).
 void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ldo, int M, int N, int K,
-               const GemmEpilogue& epi, cudaStream_t stream);
+               const GemmEpilogue& epi, cudaStream_t stream, int tile_n = 0);
 
 int device_sm_count();
 

@@ -26,6 +26,20 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// ------------------------------------------------------------------------------------------ register reallocation
+// Every warp of a warpgroup executes these together.  A 384-thread kernel is compiled for 168 registers per thread; the
+// producer warpgroup drops to 40 and each of the two consumer warpgroups grows to 232: 40 + 2 x 232 = 504 of the 512
+// registers one scheduler lane has for its three warps.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
 // ------------------------------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -67,20 +81,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug traps (the launch fails loudly) instead of hanging the GPU.  The bound is wall-clock
 // (~2 s of SM cycles), checked every 1024 failed probes, so it is independent of how long one try_wait suspends.  The
-// trap carries no printf by default: a function call between wgmma.mma_async and its wait_group makes ptxas serialise
-// the MMAs.  Build with -DN1_MBAR_DEBUG to have the timeout report its block, thread, barrier and parity first.
+// trap sits in a function of its own: with a trap instruction inline, ptxas keeps a kernel that reallocates registers
+// (setmaxnreg) at its launch-bound count everywhere, and the 256-wide GEMM tile spills.  It prints nothing by default;
+// build with -DN1_MBAR_DEBUG to have the timeout report its block, thread, barrier and parity first.
+static __device__ __noinline__ void mbar_timeout(uint32_t bar, uint32_t parity) {
+#ifdef N1_MBAR_DEBUG
+  printf("n1: mbarrier timeout block=(%d,%d) thread=%d bar=0x%x parity=%u\n", blockIdx.x, blockIdx.y, threadIdx.x, bar,
+         parity);
+#endif
+  __trap();
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 1023u) == 0 && clock64() - t0 > 4000000000LL) {
-#ifdef N1_MBAR_DEBUG
-      printf("n1: mbarrier timeout block=(%d,%d) thread=%d bar=0x%x parity=%u\n", blockIdx.x, blockIdx.y, threadIdx.x,
-             smem_u32(bar), parity);
-#endif
-      __trap();
-    }
+    if ((++spins & 1023u) == 0 && clock64() - t0 > 4000000000LL) mbar_timeout(smem_u32(bar), parity);
   }
 }
 
