@@ -311,6 +311,18 @@ int n1_op_gemm(const void* A_bf16, int lda, const void* W_bf16, int ldw, void* o
 int n1_op_ff_block(const void* x_bf16, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w1_bf16,
                    const float* b1, const void* w2_bf16, const float* b2, void* out_bf16, int ldo, int M, int cluster,
                    void* stream);
+/* NavDP decoder self- / cross-attention sublayers with their LayerNorm, one kernel each (dec_attn_block.cu), in place on
+ * the residual stream x bf16 [B * Ns * T, ldx] (trajectory n of environment e at rows (e * Ns + n) * T ..), D = 384,
+ * 8 heads of 48, T <= 64; weights bf16 contiguous, biases fp32:
+ *   sa: x += W_o MHA(LN(x) W_qkv^T + b_qkv) + b_o, w_qkv [1152, 384], attention within each trajectory, causal or not;
+ *   ca: x += W_o MHA(LN(x) W_q^T + b_q, K_e, V_e) + b_o, key j of environment e at kv[(e * mtok + j) * ldkv], its value
+ *       384 columns later, 1 <= mtok <= 64. */
+int n1_op_dec_sa_block(void* x_bf16, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w_qkv_bf16,
+                       const float* b_qkv, const void* w_o_bf16, const float* b_o, int B, int Ns, int T, int causal,
+                       void* stream);
+int n1_op_dec_ca_block(void* x_bf16, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w_q_bf16,
+                       const float* b_q, const void* w_o_bf16, const float* b_o, const void* kv_bf16, int ldkv, int mtok,
+                       int B, int Ns, int T, void* stream);
 int n1_op_layernorm(const void* x_bf16, int ldx, void* y_bf16, int ldy, const float* w, const float* b, int rows, int D,
                     float eps, int rms, void* stream);
 /* Row kernels of the NextDiT System 1 (reference: nextdit_traj.py L125-178 LuminaNextDiTBlock.forward, L352-356;

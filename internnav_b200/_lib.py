@@ -66,6 +66,10 @@ SYMBOLS = {
                            c_void_p, c_int, c_int, c_int, c_void_p]),
     "n1_op_ff_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                c_int, c_int, c_int, c_void_p]),
+    "n1_op_dec_sa_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_int, c_int, c_int, c_int, c_void_p]),
+    "n1_op_dec_ca_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "n1_op_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_float, c_int,
                                 c_void_p]),
     "n1_op_mod_norm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
@@ -276,3 +280,23 @@ def ff_block(x, ln_w, ln_b, w1, b1, w2, b2, eps=1e-5, out=None, cluster=2):
     check(lib().n1_op_ff_block(c_void_p(x.data_ptr()), x.stride(0), ptr(ln_w), ptr(ln_b), eps, ptr(w1), ptr(b1), ptr(w2),
                                ptr(b2), c_void_p(out.data_ptr()), out.stride(0), x.shape[0], cluster, stream_ptr()))
     return out
+
+
+def dec_sa_block(x, ln_w, ln_b, w_qkv, b_qkv, w_o, b_o, B, Ns, T, causal=True, eps=1e-5):
+    """In place: x += w_o-projection of per-trajectory MHA(LayerNorm(x) @ w_qkv.T + b_qkv) + b_o (NavDP decoder
+    self-attention sublayer, one fused kernel).  x bf16 [B * Ns * T, 384] view (row stride allowed)."""
+    assert x.dtype == torch.bfloat16 and x.shape == (B * Ns * T, 384) and x.stride(1) == 1
+    assert w_qkv.shape == (1152, 384) and w_o.shape == (384, 384)
+    check(lib().n1_op_dec_sa_block(c_void_p(x.data_ptr()), x.stride(0), ptr(ln_w), ptr(ln_b), float(eps), ptr(w_qkv),
+                                   ptr(b_qkv), ptr(w_o), ptr(b_o), B, Ns, T, 1 if causal else 0, stream_ptr()))
+    return x
+
+
+def dec_ca_block(x, ln_w, ln_b, w_q, b_q, w_o, b_o, kv, mtok, B, Ns, T, eps=1e-5):
+    """In place: x += w_o-projection of MHA(LayerNorm(x) @ w_q.T + b_q, K_e, V_e) + b_o (NavDP decoder cross-attention
+    sublayer, one fused kernel).  kv bf16 view [B * mtok, >= 768] (row stride allowed): K in columns 0..383, V in 384..767."""
+    assert x.dtype == torch.bfloat16 and x.shape == (B * Ns * T, 384) and x.stride(1) == 1
+    assert w_q.shape == (384, 384) and w_o.shape == (384, 384) and kv.shape[0] == B * mtok and kv.stride(1) == 1
+    check(lib().n1_op_dec_ca_block(c_void_p(x.data_ptr()), x.stride(0), ptr(ln_w), ptr(ln_b), float(eps), ptr(w_q), ptr(b_q),
+                                   ptr(w_o), ptr(b_o), c_void_p(kv.data_ptr()), kv.stride(0), mtok, B, Ns, T, stream_ptr()))
+    return x

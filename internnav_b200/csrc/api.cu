@@ -607,6 +607,20 @@ int n1_op_ff_block(const void* x, int ldx, const float* ln_w, const float* ln_b,
   });
 }
 
+int n1_op_dec_sa_block(void* x, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w_qkv,
+                       const float* b_qkv, const void* w_o, const float* b_o, int B, int Ns, int T, int causal, void* stream) {
+  return guard([&] {
+    dec_sa_block(B16(x), ldx, ln_w, ln_b, eps, B16(w_qkv), b_qkv, B16(w_o), b_o, B, Ns, T, causal, S(stream));
+  });
+}
+int n1_op_dec_ca_block(void* x, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w_q, const float* b_q,
+                       const void* w_o, const float* b_o, const void* kv, int ldkv, int mtok, int B, int Ns, int T,
+                       void* stream) {
+  return guard([&] {
+    dec_ca_block(B16(x), ldx, ln_w, ln_b, eps, B16(w_q), b_q, B16(w_o), b_o, B16(kv), ldkv, mtok, B, Ns, T, S(stream));
+  });
+}
+
 int n1_op_mod_norm(const void* x, int ldx, const float* w, const void* mod, int ld_mod, int rows_per_group, const void* res,
                    int ldr, void* out, int ldo, int64_t rows, int D, float eps, int mode, void* stream) {
   return guard([&] {

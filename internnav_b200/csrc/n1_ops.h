@@ -112,6 +112,16 @@ void attention_tc128(const AttnParams& p, cudaStream_t stream);
 // hidden activations kept on the SM.  x / out bf16 [M, ld] (may alias), w1 [1536, 384], w2 [384, 1536] contiguous.
 void ff_block_384(const bf16* x, int ldx, const float* ln_w, const float* ln_b, float eps, const bf16* w1, const float* b1,
                   const bf16* w2, const float* b2, bf16* out, int ldo, int M, int cluster, cudaStream_t stream);
+// Self- / cross-attention sublayers of the NavDP decoder layer, one kernel each (dec_attn_block.cu), in place on the
+// residual stream x [B * Ns * T, ldx] bf16 (rows of trajectory n of environment e at (e * Ns + n) * T), D = 384, 8 heads
+// of 48, T <= 64.  Weights contiguous bf16: w_qkv [1152, 384] (q | k | v), w_q / w_o [384, 384]; biases fp32.
+//   self:  x += W_o MHA(LN(x) W_qkv^T + b_qkv) + b_o, attention within each trajectory (causal: key j <= query i)
+//   cross: x += W_o MHA(LN(x) W_q^T + b_q, K_e, V_e) + b_o, K_e row j at kv[(e * mtok + j) * ldkv], V_e at + 384, mtok <= 64
+void dec_sa_block(bf16* x, int ldx, const float* ln_w, const float* ln_b, float eps, const bf16* w_qkv, const float* b_qkv,
+                  const bf16* w_o, const float* b_o, int B, int Ns, int T, int causal, cudaStream_t stream);
+void dec_ca_block(bf16* x, int ldx, const float* ln_w, const float* ln_b, float eps, const bf16* w_q, const float* b_q,
+                  const bf16* w_o, const float* b_o, const bf16* kv, int ldkv, int mtok, int B, int Ns, int T,
+                  cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------- NextDiT rows (nextdit_kernels.cu)
 // Modulated / gated norms of LuminaNextDiTBlock (nextdit_traj.py L125-178) over bf16 rows of width D <= 1024, D % 8 == 0;

@@ -394,15 +394,30 @@ struct S1Model::DenoiseBufs {
   int* klen;  // [B] visible memory-token count per environment (critic pass)
 };
 
+// Whether a sampling / eps pass over horizon T runs each decoder layer as the three fused kernels (self-attention block,
+// cross-attention block, FF block) instead of the 9-launch sequence.  The blocks cover D = 384 / 8 heads (load() checks
+// both), T <= 32, <= 64 condition tokens and contiguous weights; the critic pass (mode 2) always takes the sequence.
+bool S1Model::fused_attn(int T) const {
+  const int D = dims.D;
+  if (!loaded_ || T > 32 || dims.cond_tokens() > 64 || ff_block_mode() == 0) return false;
+  for (const DecLayer& L : dec_)
+    if (L.sa_qkv.ldw != D || L.sa_out.ldw != D || L.ca_q.ldw != D || L.ca_out.ldw != D || L.ff1.N != 1536 ||
+        L.ff1.ldw != D || L.ff2.ldw != 1536)
+      return false;
+  return true;
+}
+
 S1Model::DenoiseBufs S1Model::carve_denoise(Carver& c, int B, int Ns, int T) const {
   const int D = dims.D, Mtok = dims.cond_tokens();
   const long R = (long)B * Ns * T;
-  DenoiseBufs d;
+  DenoiseBufs d = {};
   d.x = c.take<bf16>(R * D);
   d.x2 = c.take<bf16>(R * D);  // ping-pong partner of x for the fused GEMM + LayerNorm (no in-place update there)
-  d.ln = c.take<bf16>(R * D);
-  d.qkv = c.take<bf16>(R * 3 * D);
-  d.att = c.take<bf16>(R * D);
+  if (!fused_attn(T) || dims.standalone) {  // the 9-launch layer can run (the stand-alone policy's critic pass takes it)
+    d.ln = c.take<bf16>(R * D);
+    d.qkv = c.take<bf16>(R * 3 * D);
+    d.att = c.take<bf16>(R * D);
+  }
   d.hid = c.take<bf16>(R * 4 * D);
   d.cond = c.take<bf16>((long)B * Mtok * D);
   d.ckv = c.take<bf16>((long)B * Mtok * kv_all_.N);
@@ -429,8 +444,19 @@ void S1Model::decoder_pass(const DenoiseBufs& d, const float* x_t, const int* ts
     build_cond(tsteps, t_scalar, goal, rgbd, cond_pos_, d.cond, B, Mtok, 0, 1, s, dims.goal_slots);
     linear(kv_all_, d.cond, Mtok * D, d.ckv, Mtok * ldkv, B, GemmEpilogue(), s);
   }
-  const float scale48 = 1.0f / sqrtf(48.f);
   bf16* xc = d.x;   // current residual stream
+  if (!critic && fused_attn(T)) {
+    for (int l = 0; l < dims.layers; ++l) {
+      const DecLayer& L = dec_[l];
+      dec_sa_block(xc, D, L.n1.w, L.n1.b, 1e-5f, L.sa_qkv.w, L.sa_qkv.b, L.sa_out.w, L.sa_out.b, B, Ns, T, 1, s);
+      dec_ca_block(xc, D, L.n2.w, L.n2.b, 1e-5f, L.ca_q.w, L.ca_q.b, L.ca_out.w, L.ca_out.b, d.ckv + (long)l * 2 * D, ldkv,
+                   Mtok, B, Ns, T, s);
+      ff_block_384(xc, D, L.n3.w, L.n3.b, 1e-5f, L.ff1.w, L.ff1.b, L.ff2.w, L.ff2.b, xc, D, (int)R, ff_block_mode(), s);
+    }
+    head_ddpm(xc, final_ln_.w, final_ln_.b, head_w_, head_b_, R, mode, x_io, noise, eps, cf, s);
+    return;
+  }
+  const float scale48 = 1.0f / sqrtf(48.f);
   // residual GEMM (N = 384) and the LayerNorm that follows it
   auto res_gemm_ln = [&](const Lin& W, const bf16* A, int lda, const LNp* ln) {
     GemmEpilogue res;

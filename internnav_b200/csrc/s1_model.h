@@ -123,6 +123,7 @@ class S1Model {
   size_t rgbd_impl(Carver c, const float* rgb, const float* depth, bf16* out, int B, cudaStream_t s) const;
   size_t goal_impl(Carver c, const bf16* latents, bf16* goal, int B, cudaStream_t s) const;
   DenoiseBufs carve_denoise(Carver& c, int B, int Ns, int T) const;
+  bool fused_attn(int T) const;
   void decoder_pass(const DenoiseBufs& d, const float* x_t, const int* tsteps, int t_scalar, bool cond_full,
                     const bf16* goal, const bf16* rgbd, int B, int Ns, int T, int mode, float* x_io,
                     const float* noise, float* eps, const DdpmCoef& cf, cudaStream_t s) const;
