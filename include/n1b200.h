@@ -307,10 +307,9 @@ int n1_op_gemm(const void* A_bf16, int lda, const void* W_bf16, int ldw, void* o
                void* stream);
 /* NavDP decoder FF block with its LayerNorm, residual stream resident in tensor memory (ff_block.cu):
  * out = x + W2 GELU(W1 LayerNorm(x; ln_w, ln_b, eps) + b1) + b2 -- norm3 / linear1 / GELU / linear2 / residual of
- * nn.TransformerDecoderLayer(norm_first=True), navdp.py L57-66.  x, out bf16 [M, 384] (may alias).  cluster: 1 or 2. */
+ * nn.TransformerDecoderLayer(norm_first=True), navdp.py L57-66.  x, out bf16 [M, 384] (may alias). */
 int n1_op_ff_block(const void* x_bf16, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w1_bf16,
-                   const float* b1, const void* w2_bf16, const float* b2, void* out_bf16, int ldo, int M, int cluster,
-                   void* stream);
+                   const float* b1, const void* w2_bf16, const float* b2, void* out_bf16, int ldo, int M, void* stream);
 /* NavDP decoder self- / cross-attention sublayers with their LayerNorm, one kernel each (dec_attn_block.cu), in place on
  * the residual stream x bf16 [B * Ns * T, ldx] (trajectory n of environment e at rows (e * Ns + n) * T ..), D = 384,
  * 8 heads of 48, T <= 64; weights bf16 contiguous, biases fp32:

@@ -65,7 +65,7 @@ SYMBOLS = {
     "n1_op_gemm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                            c_void_p, c_int, c_int, c_int, c_void_p]),
     "n1_op_ff_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                               c_int, c_int, c_int, c_void_p]),
+                               c_int, c_int, c_void_p]),
     "n1_op_dec_sa_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_int, c_int, c_int, c_int, c_void_p]),
     "n1_op_dec_ca_block": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -271,14 +271,14 @@ def attention_varlen(q, k, v, heads_q, heads_kv, head_dim, cu_seqlens, max_seq, 
     return o, bool(used.value)
 
 
-def ff_block(x, ln_w, ln_b, w1, b1, w2, b2, eps=1e-5, out=None, cluster=2):
+def ff_block(x, ln_w, ln_b, w1, b1, w2, b2, eps=1e-5, out=None):
     """out = x + gelu(LayerNorm(x) @ w1.T + b1) @ w2.T + b2 (NavDP decoder FF block, one fused kernel)."""
     assert x.dtype == torch.bfloat16 and x.shape[1] == 384 and w1.shape == (1536, 384) and w2.shape == (384, 1536)
     assert w1.is_contiguous() and w2.is_contiguous() and x.stride(1) == 1
     if out is None:
         out = torch.empty(x.shape[0], 384, device=x.device, dtype=torch.bfloat16)
     check(lib().n1_op_ff_block(c_void_p(x.data_ptr()), x.stride(0), ptr(ln_w), ptr(ln_b), eps, ptr(w1), ptr(b1), ptr(w2),
-                               ptr(b2), c_void_p(out.data_ptr()), out.stride(0), x.shape[0], cluster, stream_ptr()))
+                               ptr(b2), c_void_p(out.data_ptr()), out.stride(0), x.shape[0], stream_ptr()))
     return out
 
 

@@ -601,9 +601,9 @@ int n1_test_gemm(const void* A, int lda, const void* W, int ldw, void* out, int 
 }
 
 int n1_op_ff_block(const void* x, int ldx, const float* ln_w, const float* ln_b, float eps, const void* w1, const float* b1,
-                   const void* w2, const float* b2, void* out, int ldo, int M, int cluster, void* stream) {
+                   const void* w2, const float* b2, void* out, int ldo, int M, void* stream) {
   return guard([&] {
-    ff_block_384(B16(x), ldx, ln_w, ln_b, eps, B16(w1), b1, B16(w2), b2, B16(out), ldo, M, cluster, S(stream));
+    ff_block_384(B16(x), ldx, ln_w, ln_b, eps, B16(w1), b1, B16(w2), b2, B16(out), ldo, M, S(stream));
   });
 }
 

@@ -16,8 +16,7 @@
 // attention(); this file keeps the general path (any length, GQA, slotted K/V cache, head_dim 48 / 64 / 80 / 128).
 #include <stdlib.h>
 
-#include "n1_ops.h"
-#include "n1_ptx.cuh"
+#include "dec_tile.cuh"
 
 namespace n1 {
 namespace {
@@ -275,65 +274,13 @@ __global__ void __launch_bounds__(256) attn_small_kernel(const AttnParams p, con
       for (int ks = 0; ks < 3; ++ks)
         ldsm_x4(smem_u32(sQ + (mt * 16 + lr + (lm & 1) * 8) * RS + h * 96 + (ks * 16 + (lm >> 1) * 8) * 2), qf[ks][0],
                 qf[ks][1], qf[ks][2], qf[ks][3]);
-      float s[2 * NKP][4];
-#pragma unroll
-      for (int i = 0; i < 2 * NKP; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-      for (int ks = 0; ks < 3; ++ks)
-#pragma unroll
-        for (int np = 0; np < NKP; ++np) {
-          uint32_t b0, b1, b2, b3;
-          ldsm_x4(smem_u32(sK + (np * 16 + (lm >> 1) * 8 + lr) * RS + h * 96 + (ks * 16 + (lm & 1) * 8) * 2), b0, b1, b2, b3);
-          mma_bf16(s[2 * np], qf[ks], b0, b1);
-          mma_bf16(s[2 * np + 1], qf[ks], b2, b3);
-        }
       const int row_a = mt * 16 + (lane >> 2), row_b = row_a + 8;
-      float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 2 * NKP; ++i)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = i * 8 + (lane & 3) * 2 + (e & 1);
-          const int qi = e < 2 ? row_a : row_b;
-          bool vis = key < sk;
-          if (p.causal) vis = vis && key <= qi + causal_off;
-          s[i][e] = vis ? s[i][e] * sl2 : -INFINITY;
-          mx[e >> 1] = fmaxf(mx[e >> 1], s[i][e]);
-        }
-      float sum[2] = {0.f, 0.f};
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        if (mx[r] == -INFINITY) mx[r] = 0.f;
-      }
-      uint32_t pf[NKP][4];
-#pragma unroll
-      for (int i = 0; i < 2 * NKP; ++i) {
-        const float p0 = exp2f(s[i][0] - mx[0]), p1 = exp2f(s[i][1] - mx[0]);
-        const float p2 = exp2f(s[i][2] - mx[1]), p3 = exp2f(s[i][3] - mx[1]);
-        sum[0] += p0 + p1, sum[1] += p2 + p3;
-        pf[i >> 1][(i & 1) * 2 + 0] = pack_bf16(p0, p1);
-        pf[i >> 1][(i & 1) * 2 + 1] = pack_bf16(p2, p3);
-      }
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 1);
-        sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 2);
-      }
-      float o[6][4];
-#pragma unroll
-      for (int i = 0; i < 6; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-#pragma unroll
-      for (int kk = 0; kk < NKP; ++kk)
-#pragma unroll
-        for (int np = 0; np < 3; ++np) {
-          uint32_t b0, b1, b2, b3;
-          ldsm_x4_t(smem_u32(sV + (kk * 16 + (lm & 1) * 8 + lr) * RS + h * 96 + (np * 16 + (lm >> 1) * 8) * 2), b0, b1, b2, b3);
-          mma_bf16(o[2 * np], pf[kk], b0, b1);
-          mma_bf16(o[2 * np + 1], pf[kk], b2, b3);
-        }
-      const float inv0 = sum[0] > 0.f ? 1.f / sum[0] : 0.f, inv1 = sum[1] > 0.f ? 1.f / sum[1] : 0.f;
+      // key j visible to query i iff j < sk and (causal) j <= i + causal_off
+      const int lo_key[2] = {0, 0};
+      const int hi_key[2] = {p.causal ? min(sk - 1, row_a + causal_off) : sk - 1,
+                             p.causal ? min(sk - 1, row_b + causal_off) : sk - 1};
+      float o[6][4], inv0, inv1;
+      attn_hd48_16rows<NKP>(qf, sK + h * 96, sV + h * 96, RS, lo_key, hi_key, sl2, lane, o, inv0, inv1);
       // stage O over this warp's own (rows of this m-tile, head columns) slice of the Q tile: nobody else reads it
       __syncwarp();
 #pragma unroll

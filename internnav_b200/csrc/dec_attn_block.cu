@@ -14,12 +14,13 @@
 //                   input projection (slot = [q_h | k_h | v_h] rows of head h for warpgroup 0 and of head h + 4 for
 //                   warpgroup 1, 2 x 144 x 64 for self, 2 x 48 x 64 for cross), then 6 k-blocks [384 x 64] of W_o.
 //   warpgroups 0-1  consumers at 232 registers, both on the same rows; warpgroup g owns heads 4 g .. 4 g + 3:
-//       prologue    x rows -> LayerNorm -> bf16 A operand (128-byte swizzled K-major, 48 KB), as in ff_block.cu;
+//       prologue    x rows -> LayerNorm -> bf16 A operand (128-byte swizzled K-major, 48 KB), as in ff_block.cu (the
+//                   LayerNorm, the K = 384 ring loop, the attention core and the epilogue are in dec_tile.cuh);
 //       per head    projection of the head (wgmma m64n144k16 / m64n48k16, fp32), + bias, bf16.  Q stays in registers: the
 //                   accumulator layout of wgmma is the A-fragment layout of mma.sync.  K and V go to the warpgroup's
 //                   staging buffer (self: from the accumulators; cross: the environment's rows of the layer's K / V).
 //                   Each warp then runs S = Q K^T over 64 keys, the masked softmax (fp32, P rounded to bf16) and O = P V
-//                   on mma.sync.m16n8k16 for its 16 rows, exactly as attn_small_kernel (attention.cu) does, and writes
+//                   on mma.sync.m16n8k16 for its 16 rows, with attn_small_kernel's (attention.cu) code, and writes
 //                   O / rowsum as bf16 into the swizzled O tile;
 //       epilogue    y[:, 192 g ..] = O · W_o[192 g ..]^T (m64n192k16, output columns split over the warpgroups),
 //                   x = y + b_o + x -> bf16, in place (a thread re-reads exactly the elements it overwrites).
@@ -28,8 +29,7 @@
 // (rows padded from 96 to 112 bytes: conflict-free ldmatrix) | 6 mbarriers.  226 560 with the 1024-byte alignment slack.
 #include <mutex>
 
-#include "n1_ops.h"
-#include "n1_ptx.cuh"
+#include "dec_tile.cuh"
 
 namespace n1 {
 namespace {
@@ -59,7 +59,6 @@ struct DecAttnArgs {
   int causal;
 };
 
-__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory"); }
 __device__ __forceinline__ void warpgroup_barrier(int g) { asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory"); }
 
 template <bool kSelf>
@@ -88,30 +87,29 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
   if (warp >= kConsumerWarps) {
     setmaxnreg_dec<kProducerRegs>();
     if (warp == kConsumerWarps && lane == 0) {
-      int slot = 0;
-      uint32_t ph = 0;
+      Ring<kSlots> r;
       for (int t = blockIdx.x; t < args.tiles; t += gridDim.x) {
         for (int hp = 0; hp < 4; ++hp)
           for (int kb = 0; kb < D / 64; ++kb) {
-            mbar_wait(&empty[slot], ph ^ 1);
-            mbar_arrive_expect_tx(&full[slot], 2 * kHeadBytes);
-            uint8_t* dst = sW + slot * kSlotBytes;
+            mbar_wait(&empty[r.slot], r.phase ^ 1);
+            mbar_arrive_expect_tx(&full[r.slot], 2 * kHeadBytes);
+            uint8_t* dst = sW + r.slot * kSlotBytes;
 #pragma unroll
             for (int g = 0; g < 2; ++g) {
               const int h = 4 * g + hp;
 #pragma unroll
               for (int part = 0; part < NP / HD; ++part)  // q_h, k_h, v_h rows of the in_proj weight
-                tma_load_2d(dst + g * kHeadBytes + part * HD * 128, &tmIn, &full[slot], kb * 64, part * D + h * HD);
+                tma_load_2d(dst + g * kHeadBytes + part * HD * 128, &tmIn, &full[r.slot], kb * 64, part * D + h * HD);
             }
-            if (++slot == kSlots) slot = 0, ph ^= 1;
+            r.advance();
           }
         for (int kb = 0; kb < D / 64; ++kb) {
-          mbar_wait(&empty[slot], ph ^ 1);
-          mbar_arrive_expect_tx(&full[slot], kSlotBytes);
-          uint8_t* dst = sW + slot * kSlotBytes;
-          tma_load_2d(dst, &tmO, &full[slot], kb * 64, 0);
-          tma_load_2d(dst + kSlotBytes / 2, &tmO, &full[slot], kb * 64, 192);
-          if (++slot == kSlots) slot = 0, ph ^= 1;
+          mbar_wait(&empty[r.slot], r.phase ^ 1);
+          mbar_arrive_expect_tx(&full[r.slot], kSlotBytes);
+          uint8_t* dst = sW + r.slot * kSlotBytes;
+          tma_load_2d(dst, &tmO, &full[r.slot], kb * 64, 0);
+          tma_load_2d(dst + kSlotBytes / 2, &tmO, &full[r.slot], kb * 64, 192);
+          r.advance();
         }
       }
     }
@@ -121,13 +119,11 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
     const int g = cw >> 2;                          // warpgroup
     const int wtid = threadIdx.x & 127;             // thread within the warpgroup
     const int quad = lane & 3;
-    const int lm = lane >> 3, lr = lane & 7;        // ldmatrix: matrix / row of this lane's address
     const int r0 = (cw & 3) * 16 + (lane >> 2);     // this thread's accumulator rows: r0 and r0 + 8
     uint8_t* sK = sKV + g * 2 * kKvBytes;
     uint8_t* sV = sK + kKvBytes;
     const float sl2 = 0.14433756729740643f * 1.4426950408889634f;  // 48^-1/2 * log2(e)
-    int slot = 0;
-    uint32_t ph = 0;
+    Ring<kSlots> ring;
     for (int t = blockIdx.x; t < args.tiles; t += gridDim.x) {
       const int env = t / args.tiles_per_env;
       const int traj0 = (t - env * args.tiles_per_env) * args.tpt;
@@ -136,61 +132,8 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
       const int nrows = ntraj * args.T;
       // every MMA of the previous tile has completed in both warpgroups: the LN and O tiles are free
       consumer_barrier();
-      // ---- prologue: LayerNorm, one warp per 8 rows (the FF block's code); rows past the tile read as zeros
-      {
-        uint2 q[8][3];
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const int r = cw * 8 + rr;
-          const bf16* xr = args.x + (row0 + r) * args.ldx;
-#pragma unroll
-          for (int i = 0; i < 3; ++i)
-            q[rr][i] = r < nrows ? *reinterpret_cast<const uint2*>(xr + (lane + i * 32) * 4) : make_uint2(0u, 0u);
-        }
-        float s[8], sq[8];
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          s[rr] = 0.f;
-#pragma unroll
-          for (int i = 0; i < 3; ++i)
-            s[rr] += bf16_lo(q[rr][i].x) + bf16_hi(q[rr][i].x) + bf16_lo(q[rr][i].y) + bf16_hi(q[rr][i].y);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-          for (int rr = 0; rr < 8; ++rr) s[rr] += __shfl_xor_sync(0xffffffffu, s[rr], o);
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const float mu = s[rr] * (1.0f / D);
-          s[rr] = mu;
-          sq[rr] = 0.f;
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            const float a = bf16_lo(q[rr][i].x) - mu, b = bf16_hi(q[rr][i].x) - mu;
-            const float c = bf16_lo(q[rr][i].y) - mu, d = bf16_hi(q[rr][i].y) - mu;
-            sq[rr] += a * a + b * b + c * c + d * d;
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-          for (int rr = 0; rr < 8; ++rr) sq[rr] += __shfl_xor_sync(0xffffffffu, sq[rr], o);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          const int col = (lane + i * 32) * 4;
-          const float4 lw = __ldg(reinterpret_cast<const float4*>(args.ln_w + col));
-          const float4 lb = __ldg(reinterpret_cast<const float4*>(args.ln_b + col));
-          const int kb = col >> 6, ch = (col & 63) >> 3;
-#pragma unroll
-          for (int rr = 0; rr < 8; ++rr) {
-            const float mu = s[rr], rstd = rsqrtf(sq[rr] * (1.0f / D) + args.eps);
-            const float y0 = (bf16_lo(q[rr][i].x) - mu) * rstd * lw.x + lb.x, y1 = (bf16_hi(q[rr][i].x) - mu) * rstd * lw.y + lb.y;
-            const float y2 = (bf16_lo(q[rr][i].y) - mu) * rstd * lw.z + lb.z, y3 = (bf16_hi(q[rr][i].y) - mu) * rstd * lw.w + lb.w;
-            uint8_t* dst = sA + kb * 8192 + cw * 1024 + rr * 128 + ((ch ^ rr) << 4) + (col & 7) * 2;
-            *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(y0, y1), pack_bf16(y2, y3));
-          }
-        }
-      }
+      // ---- prologue: LayerNorm; rows past the tile read as zeros
+      ln384_to_tile<false>(sA, args.x, args.ldx, row0, nrows, args.ln_w, args.ln_b, args.eps, cw, lane);
       fence_proxy_async_smem();
       consumer_barrier();
 
@@ -209,23 +152,7 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
         }
         // ---- projection of head h: acc[64 x NP] = LN(x) · W_in[head rows]^T, K = 384
         float acc[NP / 2];
-        int prev = -1;
-#pragma unroll 1
-        for (int kb = 0; kb < D / 64; ++kb) {
-          mbar_wait(&full[slot], ph);
-          const uint64_t ad = wgmma_desc_sw128(smem_u32(sA + kb * 8192));
-          const uint64_t bd = wgmma_desc_sw128(smem_u32(sW + slot * kSlotBytes + g * kHeadBytes));
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_ss<0, 0>(acc, ad + 2 * k, bd + 2 * k, (kb | k) != 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
-          prev = slot;
-          if (++slot == kSlots) slot = 0, ph ^= 1;
-        }
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&empty[prev]);
+        mma_k384(acc, sA, sW, full, empty, ring, kSlotBytes, g * kHeadBytes, lane, [] {});
         // ---- + bias, bf16.  Column 8 j + 2 quad (+1) of acc[4 j ..] is part j / 6 (q, k, v) of the head.
         uint32_t qf[3][4];
 #pragma unroll
@@ -243,22 +170,9 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
           }
         }
         warpgroup_barrier(g);  // K / V of head h staged
-        // ---- S = Q K^T over 64 keys (16 x 64 per warp)
-        float s[8][4];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-        for (int ks = 0; ks < 3; ++ks)
-#pragma unroll
-          for (int np = 0; np < 4; ++np) {
-            uint32_t b0, b1, b2, b3;
-            ldsm_x4(smem_u32(sK + (np * 16 + (lm >> 1) * 8 + lr) * kKvRow + (ks * 16 + (lm & 1) * 8) * 2), b0, b1, b2, b3);
-            mma_bf16(s[2 * np], qf[ks], b0, b1);
-            mma_bf16(s[2 * np + 1], qf[ks], b2, b3);
-          }
-        // ---- mask + softmax.  Self: key j is visible to row i iff both lie in one trajectory and (causal) j <= i.
-        float mx[2] = {-INFINITY, -INFINITY};
-        int lo_key[2], hi_key[2];  // visible keys of rows r0 / r0 + 8: [lo_key, hi_key]
+        // ---- attention of this warp's 16 rows over the 64 staged keys.  Self: key j is visible to row i iff both lie in
+        // one trajectory and (causal) j <= i.  Every row sees at least one key (its own position / condition key 0).
+        int lo_key[2], hi_key[2];
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const int qi = r0 + 8 * r;
@@ -269,98 +183,22 @@ dec_attn_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant_
             lo_key[r] = 0, hi_key[r] = args.mtok - 1;
           }
         }
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int key = i * 8 + quad * 2 + (e & 1), r = e >> 1;
-            const bool vis = key >= lo_key[r] && key <= hi_key[r];
-            s[i][e] = vis ? s[i][e] * sl2 : -INFINITY;
-            mx[r] = fmaxf(mx[r], s[i][e]);
-          }
-        float sum[2] = {0.f, 0.f};
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-          mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        }
-        uint32_t pf[4][4];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float p0 = exp2f(s[i][0] - mx[0]), p1 = exp2f(s[i][1] - mx[0]);
-          const float p2 = exp2f(s[i][2] - mx[1]), p3 = exp2f(s[i][3] - mx[1]);
-          sum[0] += p0 + p1, sum[1] += p2 + p3;
-          pf[i >> 1][(i & 1) * 2 + 0] = pack_bf16(p0, p1);
-          pf[i >> 1][(i & 1) * 2 + 1] = pack_bf16(p2, p3);
-        }
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 1);
-          sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 2);
-        }
-        // ---- O = P V (16 x 48 per warp)
-        float o[6][4];
-#pragma unroll
-        for (int i = 0; i < 6; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-          for (int np = 0; np < 3; ++np) {
-            uint32_t b0, b1, b2, b3;
-            ldsm_x4_t(smem_u32(sV + (kk * 16 + (lm & 1) * 8 + lr) * kKvRow + (np * 16 + (lm >> 1) * 8) * 2), b0, b1, b2, b3);
-            mma_bf16(o[2 * np], pf[kk], b0, b1);
-            mma_bf16(o[2 * np + 1], pf[kk], b2, b3);
-          }
-        // every row sees at least one key (its own position / condition key 0), so sum >= 1
-        const float inv0 = 1.f / sum[0], inv1 = 1.f / sum[1];
+        float o[6][4], inv0, inv1;
+        attn_hd48_16rows<4>(qf, sK, sV, kKvRow, lo_key, hi_key, sl2, lane, o, inv0, inv1);
 #pragma unroll
         for (int i = 0; i < 6; ++i) {
-          const int col = h * HD + i * 8;  // 16-byte chunk (col % 64) / 8 of k-block col / 64, swizzled by row % 8
-          uint8_t* base = sO + (col >> 6) * 8192 + quad * 4;
-          const int ch = (col & 63) >> 3;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int r = r0 + 8 * hh;
-            *reinterpret_cast<uint32_t*>(base + (r >> 3) * 1024 + (r & 7) * 128 + ((ch ^ (r & 7)) << 4)) =
-                hh ? pack_bf16(o[i][2] * inv1, o[i][3] * inv1) : pack_bf16(o[i][0] * inv0, o[i][1] * inv0);
-          }
+          const int col = h * HD + i * 8 + quad * 2;
+          *reinterpret_cast<uint32_t*>(sO + sw128_offset(r0, col)) = pack_bf16(o[i][0] * inv0, o[i][1] * inv0);
+          *reinterpret_cast<uint32_t*>(sO + sw128_offset(r0 + 8, col)) = pack_bf16(o[i][2] * inv1, o[i][3] * inv1);
         }
       }
       fence_proxy_async_smem();
       consumer_barrier();  // the O tile holds all 8 heads
       // ---- output projection: y[:, 192 g ..] = O · W_o[192 g ..]^T, K = 384
       float y[96] = {};
-      int prev = -1;
-#pragma unroll 1
-      for (int kb = 0; kb < D / 64; ++kb) {
-        mbar_wait(&full[slot], ph);
-        const uint64_t ad = wgmma_desc_sw128(smem_u32(sO + kb * 8192));
-        const uint64_t bd = wgmma_desc_sw128(smem_u32(sW + slot * kSlotBytes + g * (kSlotBytes / 2)));
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_ss<0, 0>(y, ad + 2 * k, bd + 2 * k, (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
-        prev = slot;
-        if (++slot == kSlots) slot = 0, ph ^= 1;
-      }
-      wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(&empty[prev]);
+      mma_k384(y, sO, sW, full, empty, ring, kSlotBytes, g * (kSlotBytes / 2), lane, [] {});
       // ---- epilogue: x = y + b_o + x
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int r = r0 + hh * 8;
-        if (r >= nrows) continue;
-        bf16* xr = args.x + (row0 + r) * args.ldx + g * 192 + quad * 2;
-#pragma unroll
-        for (int jj = 0; jj < 24; ++jj) {
-          const uint32_t xv = *reinterpret_cast<const uint32_t*>(xr + jj * 8);
-          const float2 b = __ldg(reinterpret_cast<const float2*>(args.b_o + g * 192 + jj * 8 + quad * 2));
-          *reinterpret_cast<uint32_t*>(xr + jj * 8) =
-              pack_bf16(y[jj * 4 + 2 * hh] + bf16_lo(xv) + b.x, y[jj * 4 + 2 * hh + 1] + bf16_hi(xv) + b.y);
-        }
-      }
+      residual_epilogue_192<false>(y, args.x, args.ldx, args.x, args.ldx, args.b_o, row0, nrows, g, r0, quad);
     }
   }
 }

@@ -368,7 +368,7 @@ std::vector<ShapeAcc> g_shapes;  // per-(M, N, K) sums of the event-timed launch
 CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle) {
   return make_map(ptr, rows, cols, ld, box_rows, box_cols, swizzle);
 }
-// GEMM-class kernels in other files: counted like gemm_bf16 launches (event timing is only done for gemm_bf16)
+// Counts one GEMM-class launch: gemm_bf16 and the fused decoder kernels in other files
 void prof_count_gemm(double flops) {
   (void)flops;
   g_gemm_launches++;
@@ -376,7 +376,7 @@ void prof_count_gemm(double flops) {
 }
 
 void prof_enable(bool on) { g_prof_on = on; }
-// Event bracket for GEMM-class kernels launched outside gemm_bf16 (the fused decoder blocks): returns a ticket (< 0: off)
+// Event bracket of a GEMM-class launch (gemm_bf16 and the fused decoder blocks): returns a ticket (< 0: off)
 int prof_begin(double flops, int M, int N, int K, cudaStream_t s) {
   if (!g_prof_on.load()) return -1;
   EvPair ev{};
@@ -475,25 +475,13 @@ void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ld
     bn = cost(128) <= cost(64) ? 128 : 64;
     if ((long)N * K * 2 > kWStreamsBytes && cost(256) <= cost(bn)) bn = 256;
   }
-  EvPair ev{};
-  const bool prof = g_prof_on.load();
-  if (prof) {
-    cudaEventCreate(&ev.a);
-    cudaEventCreate(&ev.b);
-    ev.flops = 2.0 * M * (double)N * K;
-    ev.M = M, ev.N = N, ev.K = K;
-    cudaEventRecord(ev.a, stream);
-  }
-  g_gemm_launches++;
-  g_total_launches++;
+  const double flops = 2.0 * M * (double)N * K;
+  const int ticket = prof_begin(flops, M, N, K, stream);
+  prof_count_gemm(flops);
   if (bn == 256) launch<256>(A, lda, W, ldw, M, N, K, a, stream);
   else if (bn == 128) launch<128>(A, lda, W, ldw, M, N, K, a, stream);
   else launch<64>(A, lda, W, ldw, M, N, K, a, stream);
-  if (prof) {
-    cudaEventRecord(ev.b, stream);
-    std::lock_guard<std::mutex> lk(g_prof_mu);
-    g_events.push_back(ev);
-  }
+  prof_end(ticket, stream);
 }
 
 }  // namespace n1

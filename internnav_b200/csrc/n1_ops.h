@@ -111,7 +111,7 @@ void attention_tc128(const AttnParams& p, cudaStream_t stream);
 // FF block of the NavDP decoder layer in one kernel (ff_block.cu): out = x + W2 GELU(W1 LayerNorm(x) + b1) + b2 with the
 // hidden activations kept on the SM.  x / out bf16 [M, ld] (may alias), w1 [1536, 384], w2 [384, 1536] contiguous.
 void ff_block_384(const bf16* x, int ldx, const float* ln_w, const float* ln_b, float eps, const bf16* w1, const float* b1,
-                  const bf16* w2, const float* b2, bf16* out, int ldo, int M, int cluster, cudaStream_t stream);
+                  const bf16* w2, const float* b2, bf16* out, int ldo, int M, cudaStream_t stream);
 // Self- / cross-attention sublayers of the NavDP decoder layer, one kernel each (dec_attn_block.cu), in place on the
 // residual stream x [B * Ns * T, ldx] bf16 (rows of trajectory n of environment e at (e * Ns + n) * T), D = 384, 8 heads
 // of 48, T <= 64.  Weights contiguous bf16: w_qkv [1152, 384] (q | k | v), w_q / w_o [384, 384]; biases fp32.

@@ -1,5 +1,5 @@
 // Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma /
-// commit / wait), clusters, fences.  Everything here is architecture plumbing shared by the kernels in this
+// commit / wait), named barriers, fences.  Everything here is architecture plumbing shared by the kernels in this
 // directory; there is no reference counterpart (the reference ships no native code, SURVEY.md F1).
 #pragma once
 #include <cuda.h>
@@ -12,18 +12,6 @@ namespace n1 {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ------------------------------------------------------------------------------------------ register reallocation
@@ -39,6 +27,9 @@ __device__ __forceinline__ void setmaxnreg_dec() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+// Barrier among the two consumer warpgroups of such a kernel only (named barrier 1, 256 threads; the producer warps never
+// join it).
+__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -53,18 +44,6 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// One arrival on behalf of a converged warp, as a PREDICATED instruction (no branch): called by all 32 lanes, elect.sync
-// both joins the lanes (every lane's earlier work is done) and picks the one that arrives.  An `if (lane == 0) arrive`
-// compiles to a divergent region that ptxas is free to sink below hundreds of independent ALU instructions.
-__device__ __forceinline__ void mbar_arrive_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q mbarrier.arrive.shared::cta.b64 _, [%0];\n\t"
-      "}" ::"r"(smem_u32(bar))
-      : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -116,28 +95,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                                 int32_t c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, "
-      "%4}], [%2], %5;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "l"(policy)
-      : "memory");
-}
-// Multicast variant: the tile lands at the same shared-memory offset in every CTA of `cta_mask`, and each of those CTAs'
-// mbarrier (same offset) receives the complete_tx.
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0,
-                                               int32_t c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
-      "%4}], [%2], %5;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "h"(cta_mask)
       : "memory");
 }
 // 2-D tile store shared -> global (bulk group completion).
@@ -225,26 +182,6 @@ __device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t (&a)[4],
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-
 // Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle, rows of exactly 128 bytes (64 bf16), 8-row groups
 // 1024 bytes apart (SBO).  K-major operands ignore LBO; for an MN-major operand wider than 64 elements LBO is the byte
 // distance between its 64-element-wide halves.  Bit layout: PTX ISA, "Matrix descriptor format" of wgmma.
@@ -286,11 +223,6 @@ __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 // Exact-GELU 0.5 x (1 + erf(x / sqrt 2)) with erf from Abramowitz & Stegun 7.1.28,

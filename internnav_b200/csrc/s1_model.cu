@@ -2,7 +2,6 @@
 #include "s1_model.h"
 
 #include <math.h>
-#include <stdlib.h>
 
 #include <vector>
 
@@ -30,17 +29,6 @@ LNp load_ln(Arena& a, const WeightSource& ws, const std::string& prefix, cudaStr
 void linear(const Lin& L, const bf16* A, int lda, void* out, int ldo, int M, GemmEpilogue e, cudaStream_t s) {
   e.bias = L.b;
   gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
-}
-
-// N1_FF_BLOCK: 0 = LayerNorm + FF1 + FF2 as three kernels, 1 / 2 = the FF-block kernel (cluster size).  Default 1
-// (tests/test_ops_gpu.py::test_ff_block covers cluster sizes 1 and 2).
-int ff_block_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("N1_FF_BLOCK");
-    mode = e ? atoi(e) : 1;
-  }
-  return mode;
 }
 
 // torch.nn.functional.interpolate(mode="bicubic", scale_factor=s, antialias=False, align_corners=False) restated
@@ -399,7 +387,7 @@ struct S1Model::DenoiseBufs {
 // both), T <= 32, <= 64 condition tokens and contiguous weights; the critic pass (mode 2) always takes the sequence.
 bool S1Model::fused_attn(int T) const {
   const int D = dims.D;
-  if (!loaded_ || T > 32 || dims.cond_tokens() > 64 || ff_block_mode() == 0) return false;
+  if (!loaded_ || T > 32 || dims.cond_tokens() > 64) return false;
   for (const DecLayer& L : dec_)
     if (L.sa_qkv.ldw != D || L.sa_out.ldw != D || L.ca_q.ldw != D || L.ca_out.ldw != D || L.ff1.N != 1536 ||
         L.ff1.ldw != D || L.ff2.ldw != 1536)
@@ -451,7 +439,7 @@ void S1Model::decoder_pass(const DenoiseBufs& d, const float* x_t, const int* ts
       dec_sa_block(xc, D, L.n1.w, L.n1.b, 1e-5f, L.sa_qkv.w, L.sa_qkv.b, L.sa_out.w, L.sa_out.b, B, Ns, T, 1, s);
       dec_ca_block(xc, D, L.n2.w, L.n2.b, 1e-5f, L.ca_q.w, L.ca_q.b, L.ca_out.w, L.ca_out.b, d.ckv + (long)l * 2 * D, ldkv,
                    Mtok, B, Ns, T, s);
-      ff_block_384(xc, D, L.n3.w, L.n3.b, 1e-5f, L.ff1.w, L.ff1.b, L.ff2.w, L.ff2.b, xc, D, (int)R, ff_block_mode(), s);
+      ff_block_384(xc, D, L.n3.w, L.n3.b, 1e-5f, L.ff1.w, L.ff1.b, L.ff2.w, L.ff2.b, xc, D, (int)R, s);
     }
     head_ddpm(xc, final_ln_.w, final_ln_.b, head_w_, head_b_, R, mode, x_io, noise, eps, cf, s);
     return;
@@ -489,12 +477,12 @@ void S1Model::decoder_pass(const DenoiseBufs& d, const float* x_t, const int* ts
       pc.k_len = d.klen, pc.k_slot = Mtok, pc.seq_k = kv_len;   // slotted addressing: env e owns rows [e * Mtok, +kv_len)
     }
     attention(pc, s);
-    const bool ffb = ff_block_mode() > 0 && L.ff1.N == 1536 && L.ff1.ldw == D && L.ff2.ldw == 1536;
+    const bool ffb = L.ff1.N == 1536 && L.ff1.ldw == D && L.ff2.ldw == 1536;  // the weights fit the FF-block kernel
     res_gemm_ln(L.ca_out, d.att, D, ffb ? nullptr : &L.n3);  // the FF-block kernel applies norm3 itself
 
     const LNp* next_ln = l + 1 < dims.layers ? &dec_[l + 1].n1 : nullptr;  // the head applies the final LayerNorm itself
     if (ffb) {
-      ff_block_384(xc, D, L.n3.w, L.n3.b, 1e-5f, L.ff1.w, L.ff1.b, L.ff2.w, L.ff2.b, xc, D, (int)R, ff_block_mode(), s);
+      ff_block_384(xc, D, L.n3.w, L.n3.b, 1e-5f, L.ff1.w, L.ff1.b, L.ff2.w, L.ff2.b, xc, D, (int)R, s);
       if (next_ln) layernorm(xc, D, d.ln, D, next_ln->w, next_ln->b, (int)R, D, 1e-5f, 0, s);
     } else {
       GemmEpilogue gelu;

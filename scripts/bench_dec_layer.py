@@ -62,7 +62,7 @@ def layer(B, Ns, T, gen, acts, l=0):
         ("cross attention", lambda: _lib.attention(q, ckv[:, :D], ckv[:, D:], 8, 8, 48, B * Ns, T, MTOK, kv_div=Ns),
          4.0 * R * MTOK * D, 2 * act),
         ("ca_out gemm + residual", lambda: _lib.gemm(q, wo2, bias=bo2, residual=x, out=x), 2.0 * R * D * D, 3 * act),
-        ("ff block", lambda: _lib.ff_block(x, *lns[2], w1, b1, w2, b2, out=x, cluster=1), 4.0 * R * D * 1536, 2 * act),
+        ("ff block", lambda: _lib.ff_block(x, *lns[2], w1, b1, w2, b2, out=x), 4.0 * R * D * 1536, 2 * act),
         ("layernorm (next norm1)", lambda: _lib.layernorm(x, *lns[0], out=ln), 0.0, 2 * act),
     ]
     fused = [
@@ -70,7 +70,7 @@ def layer(B, Ns, T, gen, acts, l=0):
          2.0 * R * 4 * D * D + 4.0 * R * T * D, 2 * act),
         ("ca block", lambda: _lib.dec_ca_block(x, *lns[1], wq, bq, wo2, bo2, ckv, MTOK, B, Ns, T),
          2.0 * R * 2 * D * D + 4.0 * R * MTOK * D, 2 * act),
-        ("ff block", lambda: _lib.ff_block(x, *lns[2], w1, b1, w2, b2, out=x, cluster=1), 4.0 * R * D * 1536, 2 * act),
+        ("ff block", lambda: _lib.ff_block(x, *lns[2], w1, b1, w2, b2, out=x), 4.0 * R * D * 1536, 2 * act),
     ]
     return seq, fused
 

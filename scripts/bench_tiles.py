@@ -1,6 +1,5 @@
 """Developer microbenchmark of the two tensor-core kernels the benchmark spends its time in, at the benchmark's own shapes:
-every GEMM tile width (forced through _lib.gemm_tile) against the dispatcher's choice, and the fused FF block with and
-without its 2-CTA cluster.
+every GEMM tile width (forced through _lib.gemm_tile) against the dispatcher's choice, and the fused FF block.
 
     python scripts/bench_tiles.py [--repeats 7] [--out FILE.json]
 
@@ -90,7 +89,7 @@ def main():
     b1, b2 = torch.randn(1536, device="cuda"), torch.randn(384, device="cuda")
     lw, lb = torch.randn(384, device="cuda"), torch.randn(384, device="cuda")
     out = torch.empty_like(x)
-    variants = {"cluster%d" % c: (lambda c=c: _lib.ff_block(x, lw, lb, w1, b1, w2, b2, out=out, cluster=c)) for c in (1, 2)}
+    variants = {"fused": lambda: _lib.ff_block(x, lw, lb, w1, b1, w2, b2, out=out)}
     report("ff block M=%d" % FF_M, 4.0 * FF_M * 384 * 1536, time_variants(variants, args.repeats, flush), rows)
     if args.out:
         with open(args.out, "w") as fh:

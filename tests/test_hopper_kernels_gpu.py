@@ -703,12 +703,12 @@ def _ff_operands(M, seed):
     return [t.cuda() for t in (x.bfloat16(), lw, lb, w1, b1, w2, b2)]
 
 
-@pytest.mark.parametrize("cluster", [1, 2])
+@pytest.mark.parametrize("seed", [1, 2])
 @pytest.mark.parametrize("M", [1, 63, 64, 65, 129, 192])
-def test_ff_block_edges(L, M, cluster):
-    """M below, at and past the 64-row tile (M = 192: three tiles, so one CTA of the last 2-CTA cluster is idle), x and
-    out as column slices of wider buffers with sentinels around them, then in place; eps = 1e-6."""
-    x, lw, lb, w1, b1, w2, b2 = _ff_operands(M, M * 2 + cluster)
+def test_ff_block_tile_edges(L, M, seed):
+    """M below, at and past the 64-row tile, x and out as column slices of wider buffers with sentinels around them, then
+    in place; eps = 1e-6."""
+    x, lw, lb, w1, b1, w2, b2 = _ff_operands(M, M * 2 + seed)
     eps = 1e-6
     ref, bound = ff_ref(x, lw, lb, w1, b1, w2, b2, eps)
     xbuf, xv = guarded(M, D, torch.bfloat16, "cuda", left=16, right=24)
@@ -717,15 +717,15 @@ def test_ff_block_edges(L, M, cluster):
     outs = []
     for _ in range(2):
         obuf, ov = guarded(M, D, torch.bfloat16, "cuda", left=8, right=40)
-        L.ff_block(xv, lw, lb, w1, b1, w2, b2, eps=eps, out=ov, cluster=cluster)
+        L.ff_block(xv, lw, lb, w1, b1, w2, b2, eps=eps, out=ov)
         torch.cuda.synchronize()
         assert_guard(obuf, ov, "ff_block out")
         assert torch.equal(xbuf.view(torch.int16), xsnap.view(torch.int16)), "ff_block wrote into its input"
         outs.append(ov.clone())
-    assert_within(outs[0], ref, bound, "ff_block M=%d cluster=%d" % (M, cluster))
+    assert_within(outs[0], ref, bound, "ff_block M=%d seed=%d" % (M, seed))
     assert torch.equal(outs[0], outs[1]), "second call differs"
     # in place on the residual stream slice, as the decoder runs it
-    L.ff_block(xv, lw, lb, w1, b1, w2, b2, eps=eps, out=xv, cluster=cluster)
+    L.ff_block(xv, lw, lb, w1, b1, w2, b2, eps=eps, out=xv)
     torch.cuda.synchronize()
     assert_guard(xbuf, xv, "ff_block in place")
     assert torch.equal(xv, outs[0]), "in-place result differs"

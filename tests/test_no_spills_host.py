@@ -1,6 +1,8 @@
-"""The two warp-specialised tensor-core kernels that reallocate registers (setmaxnreg: producer warpgroup 40, consumer
-warpgroups 232) must compile for sm_90a without a byte of register spill.  The 256-wide GEMM tile and the FF block only fit
-because of that reallocation, and a spill in their main loops is a silent slowdown no other test would see."""
+"""The warp-specialised tensor-core kernels that reallocate registers (setmaxnreg: producer warpgroup 40, consumer
+warpgroups 232) must compile for sm_90a without a byte of register spill.  The 256-wide GEMM tile, the FF block and the
+decoder attention blocks only fit because of that reallocation, and a spill in their main loops is a silent slowdown no
+other test would see.  attn_small_kernel shares its attention core (dec_tile.cuh) with the decoder attention blocks, so a
+change made for those is checked against it too."""
 import os
 import re
 import shutil
@@ -17,7 +19,9 @@ def _nvcc():
 
 
 @pytest.mark.skipif(_nvcc() is None, reason="nvcc not installed")
-@pytest.mark.parametrize("src,kernel,entries", [("gemm_wgmma.cu", "gemm_kernel", 3), ("ff_block.cu", "ff_block_kernel", 2)])
+@pytest.mark.parametrize("src,kernel,entries", [("gemm_wgmma.cu", "gemm_kernel", 3), ("ff_block.cu", "ff_block_kernel", 1),
+                                                ("dec_attn_block.cu", "dec_attn_kernel", 2),
+                                                ("attention.cu", "attn_small_kernel", 4)])
 def test_kernels_compile_without_spills(tmp_path, src, kernel, entries):
     from internnav_b200 import build
     cmd = [_nvcc()] + build.FLAGS + ["-c", os.path.join(build.CSRC, src), "-o", str(tmp_path / "k.o")]
