@@ -196,9 +196,45 @@ int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const
                     const int32_t* eos_ids_host, int n_eos, int32_t pad_id, int32_t* tokens_host, int32_t* lens_host,
                     void* latents_bf16, int32_t* passes_host, void* stream);
 
+/* ---- continuing a conversation on its K/V cache (the look-down turn of the policy)
+ * A K/V pool is caller-owned device memory for `slots` conversations of up to `capacity` tokens each, in every decoder
+ * layer: 2 * layers * kv_heads * head_dim * 2 bytes per token (57 344 B for Qwen2.5-VL-7B).  It is sized once.
+ * n1_gen_plan_create_cont is n1_gen_plan_create over the FULL prompts and all their image grids, plus, per sequence, a
+ * pool slot and the number of leading prompt tokens whose K/V that slot already holds (0: a fresh sequence, written to
+ * the slot).  Only the remaining rows are embedded and prefilled, so image_feats covers only the images after that
+ * prefix; the prefix may not end inside an image, the slots of one batch must differ, and prompt + max_new_tokens +
+ * n_query must fit the capacity.  n1_llm_generate_pool is n1_llm_generate on such a plan; it refuses a reused length
+ * beyond the rows the slot holds (n1_kv_pool_valid), and afterwards the slot holds the prompt and every generated token
+ * whose K/V a pass wrote (all of them when latents_bf16 is given, all but the last otherwise). */
+typedef struct n1_kv_pool_s* n1_kv_pool;
+int n1_kv_pool_create(n1_handle h, int slots, int capacity, n1_kv_pool* out);
+void n1_kv_pool_destroy(n1_kv_pool p);
+size_t n1_kv_pool_bytes(n1_kv_pool p);
+int n1_kv_pool_valid(n1_kv_pool p, int slot); /* rows slot holds, or a negative error code */
+/* copies rows [row, row + n) of a slot in one layer to DEVICE buffers k_out / v_out [n, kv_heads * head_dim] bf16 */
+int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_out, void* v_out, void* stream);
+int n1_gen_plan_create_cont(n1_handle h, const int32_t* input_ids_host, const int32_t* lens_host, int B,
+                            const int32_t* grid_thw_host, int n_img, int max_new_tokens, n1_kv_pool pool,
+                            const int32_t* reused_host, const int32_t* slots_host, n1_llm_plan* out, void* stream);
+int n1_llm_generate_pool(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes,
+                         const void* image_feats_bf16, const int32_t* eos_ids_host, int n_eos, int32_t pad_id,
+                         int32_t* tokens_host, int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
+/* content digest of n_img images, image i = rows [row_off[i], row_off[i + 1]) of bf16 pixels [*, cols] (all DEVICE
+ * pointers; cols even) -> digest[i]: equal rows give equal digests, different rows differ with ~2^-64 odds */
+int n1_image_digest(const void* pixels_bf16, int64_t cols, const int64_t* row_off_dev, int n_img, uint64_t* digest_dev,
+                    void* stream);
+
 /* HOST-only integer helpers (no GPU needed): the same planners, exposed for bit-exact parity tests. */
 int n1_rope_index(const int32_t* input_ids_host, int len, const int32_t* grid_thw_host, int n_img, int merge,
                   int32_t* pos3_host /* [3, len] */, int32_t* delta_host);
+/* the row bookkeeping of a generation plan (n1_gen_plan_create, or n1_gen_plan_create_cont when reused_host / slots_host
+ * are given with a pool of pool_slots x pool_capacity rows), without a device: *n_rows planned rows, cu_host [B + 1],
+ * kind_host / src_host / dest_host [rows] (0 text / 1 image / 2 latent query, token id / feature row, K/V cache row),
+ * k_len_host [B] keys after the prefill.  Row arrays hold at most cap_rows entries. */
+int n1_plan_rows_host(const int32_t* input_ids_host, const int32_t* lens_host, int B, const int32_t* grid_thw_host,
+                      int n_img, int merge, int vocab, int n_query, int max_new_tokens, int pool_slots, int pool_capacity,
+                      const int32_t* reused_host, const int32_t* slots_host, int cap_rows, int32_t* n_rows,
+                      int32_t* cu_host, int32_t* kind_host, int32_t* src_host, int32_t* dest_host, int32_t* k_len_host);
 /* window_index_host [n_patches/merge^2]; cu_window_host: capacity >= n_patches/merge^2 + 2, count returned in *n_cu */
 int n1_vit_window_index(const int32_t* grid_thw_host, int n_img, int merge, int window, int32_t* window_index_host,
                         int32_t* cu_window_host, int32_t* n_cu, int32_t* pos_hw_host /* [n_patches, 2] or NULL */);
@@ -351,6 +387,14 @@ int n1_op_attention(const void* q, const void* k, const void* v, void* o, int ld
 int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int ldq, int ldk, int ldv, int ldo, int heads_q,
                        int heads_kv, int head_dim, int batch, const int32_t* cu_seqlens, int max_seq, int64_t total_rows,
                        int causal, float scale, int* used_tcgen05, void* stream);
+
+/* Chunk attention over a slotted K/V cache, head_dim 128 (wgmma): sequence b's query rows [cu_q[b], cu_q[b + 1]) of q are
+ * its tokens ctx[b] .. ctx[b] + n_b - 1 and attend (bottom-right causal) to keys / values at rows row0[b] ..
+ * row0[b] + ctx[b] + n_b - 1 of k / v ([kv_rows, heads_kv * 128], stride ldkv), which already hold the chunk's own K/V.
+ * cu_q / ctx / row0 int32 on the device.  The continuation prefill of n1_llm_generate_pool runs it. */
+int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
+                          void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
+                          int max_chunk, int heads_q, int heads_kv, float scale, void* stream);
 
 #ifdef __cplusplus
 }

@@ -81,6 +81,8 @@ SYMBOLS = {
                                    c_int, c_void_p, c_int, ctypes.c_int64, c_int, c_float, ctypes.POINTER(c_int), c_void_p]),
     "n1_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                 c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
+    "n1_op_attention_cache": (c_int, [c_void_p, c_int, ctypes.c_int64, c_void_p, c_void_p, c_int, ctypes.c_int64, c_void_p,
+                                      c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
 }
 
 OP_RGBD, OP_GOAL, OP_DENOISE = 1, 2, 3
@@ -269,6 +271,22 @@ def attention_varlen(q, k, v, heads_q, heads_kv, head_dim, cu_seqlens, max_seq, 
                                    cu_seqlens.numel() - 1, ptr(cu_seqlens), int(max_seq), q.shape[0], 1 if causal else 0,
                                    float(scale), ctypes.byref(used), stream_ptr()))
     return o, bool(used.value)
+
+
+def attention_cache(q, k, v, heads_q, heads_kv, cu_q, ctx, row0, max_chunk, scale=None, out=None):
+    """Chunk attention over a slotted K/V cache (head_dim 128): q [rows, >=heads_q*128] packed chunk rows (sequence b at
+    cu_q[b] .. cu_q[b + 1]), k / v [kv_rows, heads_kv*128] cache rows (sequence b's keys at row0[b] .. row0[b] + ctx[b] +
+    n_b - 1), cu_q / ctx / row0 int32 device tensors -> o [rows, heads_q*128] bf16, bottom-right causal."""
+    assert q.dtype == k.dtype == v.dtype == torch.bfloat16 and q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1
+    assert k.stride(0) == v.stride(0) and k.shape[0] == v.shape[0]
+    for t in (cu_q, ctx, row0):
+        assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
+    o = torch.empty(q.shape[0], heads_q * 128, device=q.device, dtype=torch.bfloat16) if out is None else out
+    check(lib().n1_op_attention_cache(c_void_p(q.data_ptr()), q.stride(0), q.shape[0], c_void_p(k.data_ptr()),
+                                      c_void_p(v.data_ptr()), k.stride(0), k.shape[0], ptr(o), o.stride(0), ptr(cu_q),
+                                      ptr(ctx), ptr(row0), cu_q.numel() - 1, int(max_chunk), heads_q, heads_kv,
+                                      float(128 ** -0.5 if scale is None else scale), stream_ptr()))
+    return o
 
 
 def ff_block(x, ln_w, ln_b, w1, b1, w2, b2, eps=1e-5, out=None):

@@ -8,6 +8,7 @@
 #include "resize.h"
 #include "bwd_kernels.h"
 #include "s1_model.h"
+#include "s2_kernels.h"
 #include "s2_model.h"
 #include "weights.h"
 
@@ -23,6 +24,9 @@ struct n1_vit_plan_s {
 };
 struct n1_llm_plan_s {
   LlmPlan* p;
+};
+struct n1_kv_pool_s {
+  KvPool* p;
 };
 struct n1_resize_plan_s {
   ResizePlan* p;
@@ -344,6 +348,86 @@ int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const
   });
 }
 
+int n1_kv_pool_create(n1_handle h, int slots, int capacity, n1_kv_pool* out) {
+  return guard([&] {
+    use(h);
+    if (!out || slots <= 0 || capacity <= 0) throw Error(N1_ERR_ARG, "n1_kv_pool_create: bad arguments");
+    n1_kv_pool_s* w = new n1_kv_pool_s();
+    try {
+      w->p = h->s2.make_pool(slots, capacity);
+    } catch (...) {
+      delete w;
+      throw;
+    }
+    *out = w;
+  });
+}
+void n1_kv_pool_destroy(n1_kv_pool p) {
+  if (!p) return;
+  delete p->p;
+  delete p;
+}
+size_t n1_kv_pool_bytes(n1_kv_pool p) { return p ? p->p->bytes() : 0; }
+int n1_kv_pool_valid(n1_kv_pool p, int slot) {
+  int r = 0;
+  const int e = guard([&] {
+    if (!p) throw Error(N1_ERR_ARG, "null pool");
+    if (slot < 0 || slot >= p->p->slots) throw Error(N1_ERR_ARG, "n1_kv_pool_valid: slot out of range");
+    r = p->p->valid[slot];
+  });
+  return e == N1_OK ? r : e;
+}
+int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_out, void* v_out, void* stream) {
+  return guard([&] {
+    if (!p || !k_out || !v_out) throw Error(N1_ERR_ARG, "null pool / buffer");
+    const KvPool& q = *p->p;
+    if (layer < 0 || layer >= q.layers || slot < 0 || slot >= q.slots || row < 0 || n < 0 || row + n > q.cap)
+      throw Error(N1_ERR_ARG, "n1_kv_pool_read: layer / slot / rows out of range");
+    const long w = q.layer_stride / ((long)q.slots * q.cap);  // kv_heads * head_dim
+    const long off = layer * q.layer_stride + ((long)slot * q.cap + row) * w;
+    N1_CUDA(cudaMemcpyAsync(k_out, q.k + off, (size_t)n * w * sizeof(bf16), cudaMemcpyDeviceToDevice, S(stream)));
+    N1_CUDA(cudaMemcpyAsync(v_out, q.v + off, (size_t)n * w * sizeof(bf16), cudaMemcpyDeviceToDevice, S(stream)));
+  });
+}
+int n1_gen_plan_create_cont(n1_handle h, const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
+                            int max_new_tokens, n1_kv_pool pool, const int32_t* reused, const int32_t* slots,
+                            n1_llm_plan* out, void* stream) {
+  return guard([&] {
+    use(h);
+    if (!ids || !lens || B <= 0 || !out || max_new_tokens < 1 || !pool || !reused || !slots)
+      throw Error(N1_ERR_ARG, "n1_gen_plan_create_cont: bad arguments");
+    n1_llm_plan_s* w = new n1_llm_plan_s();
+    try {
+      w->p = h->s2.make_llm_plan(ids, lens, B, grid, n_img, S(stream), max_new_tokens, reused, slots, pool->p);
+    } catch (...) {
+      delete w;
+      throw;
+    }
+    *out = w;
+  });
+}
+int n1_llm_generate_pool(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes, const void* image_feats,
+                         const int32_t* eos, int n_eos, int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents,
+                         int32_t* passes, void* stream) {
+  return guard([&] {
+    use(h);
+    if (!p || !pool) throw Error(N1_ERR_ARG, "null plan / pool");
+    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_pool: 0..4 eos ids");
+    GenResult r;
+    r.tokens = tokens, r.lens = lens;
+    h->s2.llm_generate_pool(*p->p, *pool->p, ws, ws_bytes, B16(image_feats), eos, n_eos, pad_id, r, B16(latents),
+                            S(stream));
+    if (passes) *passes = r.steps;
+  });
+}
+int n1_image_digest(const void* pixels, int64_t cols, const int64_t* row_off, int n_img, uint64_t* digest, void* stream) {
+  return guard([&] {
+    if ((n_img > 0 && (!pixels || !row_off || !digest)) || n_img < 0 || cols <= 0)
+      throw Error(N1_ERR_ARG, "n1_image_digest: bad arguments");
+    image_digest(B16(pixels), cols, row_off, n_img, digest, S(stream));
+  });
+}
+
 int n1_resize_plan_create(int in_h, int in_w, int out_h, int out_w, n1_resize_plan* out, void* stream) {
   return guard([&] {
     if (!out || in_h <= 0 || in_w <= 0 || out_h <= 0 || out_w <= 0) throw Error(N1_ERR_ARG, "n1_resize_plan_create: bad sizes");
@@ -526,6 +610,27 @@ int n1_op_adamw(void* master, void* working, const void* grad, void* m, void* v,
   });
 }
 
+int n1_plan_rows_host(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img, int merge, int vocab,
+                      int n_query, int max_new_tokens, int pool_slots, int pool_capacity, const int32_t* reused,
+                      const int32_t* slots, int cap_rows, int32_t* n_rows, int32_t* cu, int32_t* kind, int32_t* src,
+                      int32_t* dest, int32_t* k_len) {
+  return guard([&] {
+    if (!ids || !lens || B <= 0 || max_new_tokens < 1 || !n_rows || !cu || !kind || !src || !dest || !k_len ||
+        (!reused) != (!slots))
+      throw Error(N1_ERR_ARG, "n1_plan_rows_host: bad arguments");
+    PlanArgs a;
+    a.merge = merge, a.vocab = vocab, a.n_query = n_query, a.max_new = max_new_tokens;
+    a.ctx = reused, a.slots = slots, a.pool_slots = pool_slots, a.pool_cap = pool_capacity;
+    PlanRows r;
+    plan_rows(ids, lens, B, grid, n_img, a, r);
+    const int rows = r.cu.back();
+    if (rows > cap_rows) throw Error(N1_ERR_ARG, "n1_plan_rows_host: cap_rows < " + std::to_string(rows));
+    *n_rows = rows;
+    std::copy(r.cu.begin(), r.cu.end(), cu);
+    std::copy(r.kind.begin(), r.kind.end(), kind), std::copy(r.src.begin(), r.src.end(), src);
+    std::copy(r.dest.begin(), r.dest.end(), dest), std::copy(r.len.begin(), r.len.end(), k_len);
+  });
+}
 int n1_rope_index(const int32_t* ids, int len, const int32_t* grid, int n_img, int merge, int32_t* pos3,
                   int32_t* delta) {
   return guard([&] {
@@ -670,6 +775,19 @@ int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int
     p.kv_div = 1, p.causal = causal, p.scale = scale;
     if (used_tcgen05) *used_tcgen05 = attention_uses_tc(p) ? 1 : 0;
     attention(p, S(stream));
+  });
+}
+
+int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
+                          void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
+                          int max_chunk, int heads_q, int heads_kv, float scale, void* stream) {
+  return guard([&] {
+    if (!q || !k || !v || !o || !cu_q || !ctx || !row0) throw Error(N1_ERR_ARG, "n1_op_attention_cache: null pointer");
+    CacheAttnParams a = {};
+    a.q = B16(q), a.ldq = ldq, a.q_rows = q_rows, a.k = B16(k), a.v = B16(v), a.ldkv = ldkv, a.kv_rows = kv_rows;
+    a.o = B16(o), a.ldo = ldo, a.cu_q = cu_q, a.ctx = ctx, a.row0 = row0;
+    a.batch = batch, a.max_chunk = max_chunk, a.heads_q = heads_q, a.heads_kv = heads_kv, a.scale = scale;
+    attention_cache(a, S(stream));
   });
 }
 

@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
   const int q0 = qt * BQ;
   if (q0 >= sq) return;
   const int kb = b / p.kv_div;
-  const int k_start = p.k_len ? kb * p.k_slot : (p.cu_k ? p.cu_k[kb] : kb * p.seq_k);
+  const int k_start = p.k_len ? (p.k_row0 ? p.k_row0[kb] : kb * p.k_slot) : (p.cu_k ? p.cu_k[kb] : kb * p.seq_k);
   const int sk = p.k_len ? p.k_len[kb] : (p.cu_k ? p.cu_k[kb + 1] - k_start : p.seq_k);
   const int hk = h / (p.heads_q / p.heads_kv);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

@@ -368,6 +368,20 @@ std::vector<ShapeAcc> g_shapes;  // per-(M, N, K) sums of the event-timed launch
 CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle) {
   return make_map(ptr, rows, cols, ld, box_rows, box_cols, swizzle);
 }
+CUtensorMap tma_map_3d_sw128(const bf16* ptr, const long dims[3], const long strides[2], const int box[3]) {
+  N1_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && strides[0] % 8 == 0 && strides[1] % 8 == 0,
+           "tma_map_3d_sw128: 16-byte alignment");
+  CUtensorMap m;
+  cuuint64_t gdim[3] = {(cuuint64_t)dims[0], (cuuint64_t)dims[1], (cuuint64_t)dims[2]};
+  cuuint64_t gstr[2] = {(cuuint64_t)strides[0] * 2, (cuuint64_t)strides[1] * 2};
+  cuuint32_t bx[3] = {(cuuint32_t)box[0], (cuuint32_t)box[1], (cuuint32_t)box[2]};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(ptr), gdim, gstr, bx, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) throw Error(-5, "cuTensorMapEncodeTiled (3-D) failed: " + std::to_string((int)r));
+  return m;
+}
 // Counts one GEMM-class launch: gemm_bf16 and the fused decoder kernels in other files
 void prof_count_gemm(double flops) {
   (void)flops;

@@ -59,6 +59,9 @@ int device_sm_count();
 // 2-D bf16 tensor map over a row-major [rows, cols] matrix (leading dimension ld elements); box = [box_rows, box_cols];
 // operand tiles use box_cols = 64 with the 128-byte swizzle, output staging tiles are unswizzled.
 CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle);
+// 3-D bf16 tensor map with the 128-byte swizzle: dims innermost first, strides (elements) of dims 1 and 2, box innermost
+// first (box[0] * 2 = 128 bytes)
+CUtensorMap tma_map_3d_sw128(const bf16* ptr, const long dims[3], const long strides[2], const int box[3]);
 void prof_count_gemm(double flops);  // launch + FLOP accounting for GEMM-class kernels outside gemm_wgmma.cu
 
 // Launch accounting (always on) and optional per-GEMM event timing (bench.py's roofline pass).
@@ -99,6 +102,8 @@ struct AttnParams {
   int k_slot;            //   [kb * k_slot, kb * k_slot + k_len[kb]); overrides cu_k / seq_k
   long total_rows;       // optional: rows of the packed q / k / v buffers (var-len self-attention); > 0 lets head_dim 128
                          //   sequences of <= 320 tokens take the wgmma kernel (attention_wgmma.cu), which needs it for TMA
+  const int* k_row0;     // optional with k_len: [batch_kv] first cache row of sequence kb, replacing kb * k_slot (a
+                         //   sequence that lives in a slot of a caller-owned K/V pool)
 };
 void attention(const AttnParams& p, cudaStream_t stream);
 // wgmma / TMA attention for head_dim 128, var-len self-attention with <= 320 keys per sequence (attention_wgmma.cu)
@@ -106,6 +111,25 @@ bool attention_tc_supported(const AttnParams& p);
 // whether attention(p) runs the wgmma kernel: supported arguments and not disabled by N1_ATTN_TC=0
 bool attention_uses_tc(const AttnParams& p);
 void attention_tc128(const AttnParams& p, cudaStream_t stream);
+
+// Chunk attention over a slotted K/V cache (attention_cache_wgmma.cu), head_dim 128: sequence b has query rows
+// [cu_q[b], cu_q[b + 1]) of q (its tokens ctx[b] .. ctx[b] + n_b - 1) and keys / values at rows row0[b] .. row0[b] +
+// ctx[b] + n_b - 1 of k / v (the cache already holds the chunk's own K/V).  Bottom-right causal mask.  ctx[b] = 0 is a
+// plain prefill.  Rows past ctx[b] + n_b of a slot are never read.
+struct CacheAttnParams {
+  const bf16* q;
+  int ldq;
+  long q_rows;           // rows of the q buffer (TMA bound)
+  const bf16 *k, *v;     // [kv_rows, heads_kv * 128], row stride ldkv
+  int ldkv;
+  long kv_rows;
+  bf16* o;
+  int ldo;
+  const int *cu_q, *ctx, *row0;  // device: [batch + 1], [batch], [batch]
+  int batch, max_chunk, heads_q, heads_kv;
+  float scale;
+};
+void attention_cache(const CacheAttnParams& p, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------- fused decoder blocks
 // FF block of the NavDP decoder layer in one kernel (ff_block.cu): out = x + W2 GELU(W1 LayerNorm(x) + b1) + b2 with the

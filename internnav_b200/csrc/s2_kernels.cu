@@ -90,13 +90,13 @@ __global__ void build_embeds_kernel(const int* __restrict__ kind, const int* __r
 // in-sequence indices idx = len + gen - back + j, j in [0, per_seq): their cache rows, rotary positions (text tokens
 // after the prompt sit at idx + delta on all three mrope axes, rope2d.py L150-160) and the visible key count.
 __global__ void gen_rows_kernel(const int* __restrict__ len, const int* __restrict__ delta, const int* __restrict__ gen,
-                                int back, int per_seq, int B, int slot, int* __restrict__ dest_rows,
-                                int* __restrict__ pos3, int* __restrict__ k_len) {
+                                int back, int per_seq, int B, int slot, const int* __restrict__ row0,
+                                int* __restrict__ dest_rows, int* __restrict__ pos3, int* __restrict__ k_len) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * per_seq) return;
   const int b = i / per_seq, j = i % per_seq;
   const int idx = len[b] + gen[b] - back + j;
-  dest_rows[i] = b * slot + idx;
+  dest_rows[i] = (row0 ? row0[b] : b * slot) + idx;
   const int rows = B * per_seq;
   pos3[i] = pos3[rows + i] = pos3[2 * rows + i] = idx + delta[b];
   if (j == per_seq - 1) k_len[b] = idx + 1;
@@ -166,6 +166,26 @@ __global__ void gen_update_kernel(const int* __restrict__ next, int* __restrict_
   else atomicAdd(n_active, 1);
 }
 
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+// one CTA per image; a sum of per-word hashes, so the reduction order does not matter
+__global__ void __launch_bounds__(256) image_digest_kernel(const uint32_t* __restrict__ words, long words_per_row,
+                                                           const int64_t* __restrict__ row_off, uint64_t* __restrict__ out) {
+  const long w0 = row_off[blockIdx.x] * words_per_row, n = (row_off[blockIdx.x + 1] - row_off[blockIdx.x]) * words_per_row;
+  uint64_t h = 0;
+  for (long j = threadIdx.x; j < n; j += 256) h += splitmix64(((uint64_t)j << 32) | words[w0 + j]);
+  for (int o = 16; o > 0; o >>= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+  __shared__ unsigned long long acc;
+  if (threadIdx.x == 0) acc = (unsigned long long)n;
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) atomicAdd(&acc, (unsigned long long)h);
+  __syncthreads();
+  if (threadIdx.x == 0) out[blockIdx.x] = acc;
+}
+
 inline int nblk(long n) { return (int)((n + 255) / 256); }
 
 }  // namespace
@@ -202,9 +222,10 @@ void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, con
   N1_CUDA(cudaGetLastError());
 }
 
-void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, int* dest_rows,
-              int* pos3, int* k_len, cudaStream_t s) {
-  gen_rows_kernel<<<nblk((long)B * per_seq), 256, 0, s>>>(len, delta, gen, back, per_seq, B, slot, dest_rows, pos3, k_len);
+void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, const int* row0,
+              int* dest_rows, int* pos3, int* k_len, cudaStream_t s) {
+  gen_rows_kernel<<<nblk((long)B * per_seq), 256, 0, s>>>(len, delta, gen, back, per_seq, B, slot, row0, dest_rows, pos3,
+                                                          k_len);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }
@@ -235,6 +256,14 @@ void gen_update(const int* next, int* cur_tok, int* gen, int* finished, int* out
   N1_CUDA(cudaMemsetAsync(n_active, 0, sizeof(int), s));
   gen_update_kernel<<<nblk(B), 256, 0, s>>>(next, cur_tok, gen, finished, out_tokens, max_new, e[0], e[1], e[2], e[3], B,
                                             n_active);
+  prof_count_launch();
+  N1_CUDA(cudaGetLastError());
+}
+
+void image_digest(const bf16* pixels, long cols, const int64_t* row_off, int n_img, uint64_t* digest, cudaStream_t s) {
+  N1_CHECK(cols % 2 == 0 && n_img >= 0, "image_digest: cols must be even");
+  if (n_img == 0) return;
+  image_digest_kernel<<<n_img, 256, 0, s>>>(reinterpret_cast<const uint32_t*>(pixels), cols / 2, row_off, digest);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }

@@ -20,10 +20,11 @@ void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, con
                   const bf16* latent_queries, bf16* out, long tokens, int H, cudaStream_t s);
 
 // ---- greedy decode with a KV cache (model.generate of internvla_n1_policy.py L169-176, then generate_latents reusing it)
-// Chunk bookkeeping: per sequence the tokens idx = len + gen - back + j (j < per_seq) -> cache rows b * slot + idx,
+// Chunk bookkeeping: per sequence the tokens idx = len + gen - back + j (j < per_seq) -> cache rows b * slot + idx
+// (row0[b] + idx when row0 is given: a slot of a K/V pool),
 // mrope positions idx + delta on all three axes ([3, B * per_seq]), k_len[b] = last idx + 1.
-void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, int* dest_rows,
-              int* pos3, int* k_len, cudaStream_t s);
+void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, const int* row0,
+              int* dest_rows, int* pos3, int* k_len, cudaStream_t s);
 // cache_k/v[dest_rows[r], :] = qkv[r, k_off / v_off : + kvdim]
 void kv_append(const bf16* qkv, int ld, int k_off, int v_off, int kvdim, const int* dest_rows, long rows, bf16* cache_k,
                bf16* cache_v, cudaStream_t s);
@@ -34,5 +35,10 @@ void argmax_rows(const bf16* logits, long ld, int n, int rows, int* out, cudaStr
 // Append next[b] to every unfinished sequence; eos (host array, <= 4 ids) or gen == max_new finishes it.
 void gen_update(const int* next, int* cur_tok, int* gen, int* finished, int* out_tokens, int max_new, const int* eos_host,
                 int n_eos, int B, int* n_active, cudaStream_t s);
+
+// Content digest of n_img images: image i is rows [row_off[i], row_off[i + 1]) of a bf16 [*, cols] matrix (device
+// pointers; cols even).  digest[i] = sum over its 32-bit words w at index j of splitmix64(j << 32 | w), plus the word
+// count: equal rows give equal digests, and any change of a value or of the row count changes it but with ~2^-64 odds.
+void image_digest(const bf16* pixels, long cols, const int64_t* row_off, int n_img, uint64_t* digest, cudaStream_t s);
 
 }  // namespace n1

@@ -234,75 +234,53 @@ VitPlan* S2Model::make_vit_plan(const int32_t* grid, int n_img, cudaStream_t s) 
   return p.release();
 }
 
+KvPool::~KvPool() { cudaFree(k), cudaFree(v); }
+
+KvPool* S2Model::make_pool(int slots, int cap) const {
+  N1_CHECK(loaded_, "System-2 weights not loaded");
+  N1_CHECK(slots > 0 && cap > 0 && (long)slots * cap < (1L << 31), "kv pool: slots and capacity must be positive");
+  std::unique_ptr<KvPool> p(new KvPool());
+  p->slots = slots, p->cap = cap, p->layers = dims.layers;
+  p->layer_stride = (long)slots * cap * dims.kv_heads * dims.head_dim;
+  p->valid.assign(slots, 0);
+  N1_CUDA(cudaMalloc(&p->k, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
+  N1_CUDA(cudaMalloc(&p->v, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
+  return p.release();
+}
+
 LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
-                                cudaStream_t s, int max_new_tokens) const {
+                                cudaStream_t s, int max_new_tokens, const int32_t* ctx_in, const int32_t* slot_in,
+                                const KvPool* pool) const {
   N1_CHECK(loaded_, "System-2 weights not loaded");
   N1_CHECK(max_new_tokens != 0, "generation plan: max_new_tokens must be >= 1");
+  const bool cont = pool != nullptr;
+  N1_CHECK(cont == (ctx_in != nullptr) && cont == (slot_in != nullptr), "continuation plan: ctx, slots and pool go together");
+  N1_CHECK(!cont || max_new_tokens > 0, "continuation plan: only generation plans continue a cache");
   std::unique_ptr<LlmPlan> p(new LlmPlan());
-  const bool gen = max_new_tokens > 0;
-  const int nq = gen ? 0 : dims.n_query, unit = dims.v_merge * dims.v_merge;
-  p->B = B, p->n_query = dims.n_query;
-  std::vector<int> kind, src, out_rows, pos_all;
-  p->h_cu.push_back(0);
-  int cursor = 0;
-  long img_tok = 0, off = 0;
-  std::vector<std::vector<int>> pos_seq(B);
-  for (int b = 0; b < B; ++b) {
-    const int len = lens[b];
-    N1_CHECK(len > 0, "empty prompt");
-    std::vector<int> seq(ids + off, ids + off + len);
-    off += len;
-    for (int q = 0; q < nq; ++q) seq.push_back(kTrajTokenId);  // internvla_n1.py L327
-    const int L = (int)seq.size();
-    int delta = 0;
-    rope_index_one(seq.data(), L, grid, n_img, dims.v_merge, cursor, pos_seq[b], delta);
-    p->h_delta.push_back(delta);
-    for (int i = 0; i < L; ++i) {
-      if (i >= len) {
-        kind.push_back(2), src.push_back(i - len);  // latent_queries[q]
-        out_rows.push_back((int)kind.size() - 1);
-      } else if (seq[i] == kImageTokenId) {
-        kind.push_back(1), src.push_back((int)img_tok++);  // image features in order (L332: text_embeds[image_idx] = ...)
-      } else {
-        N1_CHECK(seq[i] >= 0 && seq[i] < dims.vocab, "token id out of vocabulary");
-        kind.push_back(0), src.push_back(seq[i]);
-      }
-    }
-    if (gen) out_rows.push_back((int)kind.size() - 1);  // logits of the last prompt token start the decode
-    p->h_cu.push_back(p->h_cu.back() + L);
-    p->max_len = std::max(p->max_len, L);
-  }
+  PlanArgs a;
+  a.merge = dims.v_merge, a.vocab = dims.vocab, a.n_query = dims.n_query, a.max_new = max_new_tokens;
+  a.ctx = ctx_in, a.slots = slot_in;
+  if (cont) a.pool_slots = pool->slots, a.pool_cap = pool->cap;
+  PlanRows r;
+  plan_rows(ids, lens, B, grid, n_img, a, r);
+  p->B = B, p->n_query = dims.n_query, p->pool = pool;
+  p->h_cu = std::move(r.cu), p->h_pos3 = std::move(r.pos3), p->h_delta = std::move(r.delta);
   p->tokens = p->h_cu.back();
-  p->n_image_tokens = img_tok;
-  p->n_out = (int)out_rows.size();
-  long expect = 0;
-  for (int i = 0; i < cursor; ++i) expect += (long)grid[i * 3] * grid[i * 3 + 1] * grid[i * 3 + 2] / unit;
-  N1_CHECK(expect == img_tok, "Image features and image tokens do not match: tokens " + std::to_string(img_tok) +
-                                  ", features " + std::to_string(expect));  // same check as internvla_n1.py L135-138
-  // [3, tokens] layout over the packed batch
-  p->h_pos3.assign((size_t)3 * p->tokens, 0);
-  for (int b = 0; b < B; ++b) {
-    const int L = p->h_cu[b + 1] - p->h_cu[b];
-    for (int st = 0; st < 3; ++st)
-      for (int i = 0; i < L; ++i) p->h_pos3[(size_t)st * p->tokens + p->h_cu[b] + i] = pos_seq[b][(size_t)st * L + i];
-  }
+  p->n_image_tokens = r.n_image_tokens;
+  p->n_out = (int)r.out_rows.size();
+  p->max_len = r.max_len;
+  if (max_new_tokens > 0) p->max_new = max_new_tokens, p->slot = r.slot;
+  if (cont) p->h_ctx = r.ctx, p->h_slot = r.slot_of, p->h_len = r.len, p->any_ctx = r.any_ctx;
   const int half = dims.head_dim / 2;
-  std::vector<int> dest, len_v;
-  if (gen) {
-    p->max_new = max_new_tokens;
-    p->slot = p->max_len + max_new_tokens + dims.n_query;
-    dest.resize(p->tokens), len_v.resize(B);
-    for (int b = 0; b < B; ++b) {
-      len_v[b] = p->h_cu[b + 1] - p->h_cu[b];
-      for (int i = 0; i < len_v[b]; ++i) dest[p->h_cu[b] + i] = b * p->slot + i;
-    }
-  }
-  // one pooled block: [ints: cu | kind | src | out_rows | pos3 | dest | len | delta] [rope table]; one H2D copy from the
-  // block's pinned twin, one kernel, no allocation / free / synchronisation once the pool holds a block of this size
-  const std::vector<int>* parts[8] = {&p->h_cu, &kind, &src, &out_rows, &p->h_pos3, &dest, &len_v, &p->h_delta};
-  size_t off_i[9] = {0};
-  for (int i = 0; i < 8; ++i) off_i[i + 1] = off_i[i] + ((parts[i]->size() + 3) & ~size_t(3));  // 16-byte aligned parts
-  const size_t int_bytes = (off_i[8] * sizeof(int) + 255) & ~size_t(255);
+  // one pooled block: [ints: cu | kind | src | out_rows | pos3 | dest | len | delta | ctx | row0] [rope table]; one H2D
+  // copy from the block's pinned twin, one kernel, no allocation / free / synchronisation once the pool holds a block of
+  // this size
+  constexpr int kParts = 10;
+  const std::vector<int>* parts[kParts] = {&p->h_cu, &r.kind, &r.src, &r.out_rows, &p->h_pos3, &r.dest, &r.len, &p->h_delta,
+                                           &r.ctx, &r.row0};
+  size_t off_i[kParts + 1] = {0};
+  for (int i = 0; i < kParts; ++i) off_i[i + 1] = off_i[i] + ((parts[i]->size() + 3) & ~size_t(3));  // 16-byte aligned
+  const size_t int_bytes = (off_i[kParts] * sizeof(int) + 255) & ~size_t(255);
   const size_t need = int_bytes + (size_t)p->tokens * half * sizeof(float2);
   PlanBlock blk = pool_take(need);
   p->block = blk.dev, p->block_bytes = blk.bytes, p->last_use = blk.last_use;
@@ -313,13 +291,14 @@ LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, 
   N1_CUDA(cudaStreamWaitEvent(s, blk.last_use, 0));  // the previous owner's consumers (any stream) are done before we overwrite
   N1_CUDA(cudaEventSynchronize(blk.last_use));       // ... and before the pinned twin is rewritten (no-op unless just recycled)
   int* hp = static_cast<int*>(blk.host);
-  for (int i = 0; i < 8; ++i)
+  for (int i = 0; i < kParts; ++i)
     if (!parts[i]->empty()) memcpy(hp + off_i[i], parts[i]->data(), parts[i]->size() * sizeof(int));
-  N1_CUDA(cudaMemcpyAsync(blk.dev, blk.host, off_i[8] * sizeof(int), cudaMemcpyHostToDevice, s));
+  N1_CUDA(cudaMemcpyAsync(blk.dev, blk.host, off_i[kParts] * sizeof(int), cudaMemcpyHostToDevice, s));
   int* dp = static_cast<int*>(blk.dev);
   p->cu = dp + off_i[0], p->kind = dp + off_i[1], p->src = dp + off_i[2], p->out_rows = dp + off_i[3];
   int* pos = dp + off_i[4];
-  if (gen) p->dest_rows = dp + off_i[5], p->d_len = dp + off_i[6], p->d_delta = dp + off_i[7];
+  if (max_new_tokens > 0) p->dest_rows = dp + off_i[5], p->d_len = dp + off_i[6], p->d_delta = dp + off_i[7];
+  if (cont) p->ctx = dp + off_i[8], p->row0 = dp + off_i[9];
   p->rope = reinterpret_cast<float2*>(static_cast<uint8_t*>(blk.dev) + int_bytes);
   mrope_table(pos, p->rope, p->tokens, half, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
   N1_CUDA(cudaEventCreateWithFlags(&p->ready, cudaEventDisableTiming));
@@ -409,13 +388,25 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
     if (kv)  // keep the rotated keys and the values of every prompt token for the decode passes
       kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, dims.kv_heads * hd, p.dest_rows, T,
                 kv->k + l * kv->layer_stride, kv->v + l * kv->layer_stride, s);
-    AttnParams a = {};
-    a.q = qkv, a.k = qkv + (long)dims.heads * hd, a.v = qkv + (long)(dims.heads + dims.kv_heads) * hd, a.o = att;
-    a.ldq = a.ldk = a.ldv = qkv_n, a.ldo = H;
-    a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
-    a.batch = p.B, a.cu_q = a.cu_k = p.cu, a.max_seq_q = p.max_len, a.total_rows = T;
-    a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
-    attention(a, s);
+    if (p.any_ctx) {  // continued sequences: the chunk attends to its slot's cached rows (which now include its own)
+      CacheAttnParams a = {};
+      a.q = qkv, a.ldq = qkv_n, a.q_rows = T;
+      a.k = kv->k + l * kv->layer_stride, a.v = kv->v + l * kv->layer_stride, a.ldkv = dims.kv_heads * hd;
+      a.kv_rows = (long)p.pool->slots * p.pool->cap;
+      a.o = att, a.ldo = H;
+      a.cu_q = p.cu, a.ctx = p.ctx, a.row0 = p.row0;
+      a.batch = p.B, a.max_chunk = p.max_len, a.heads_q = dims.heads, a.heads_kv = dims.kv_heads;
+      a.scale = 1.0f / sqrtf((float)hd);
+      attention_cache(a, s);
+    } else {
+      AttnParams a = {};
+      a.q = qkv, a.k = qkv + (long)dims.heads * hd, a.v = qkv + (long)(dims.heads + dims.kv_heads) * hd, a.o = att;
+      a.ldq = a.ldk = a.ldv = qkv_n, a.ldo = H;
+      a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
+      a.batch = p.B, a.cu_q = a.cu_k = p.cu, a.max_seq_q = p.max_len, a.total_rows = T;
+      a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
+      attention(a, s);
+    }
     GemmEpilogue res;
     res.residual = x, res.ldr = H;
     if (l == dims.layers - 1) {
@@ -493,7 +484,7 @@ void S2Model::chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, 
     a.q = g.qkv, a.k = ck, a.v = cv, a.o = g.att;
     a.ldq = qkv_n, a.ldk = a.ldv = kvd, a.ldo = H;
     a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
-    a.batch = p.B, a.seq_q = per_seq, a.k_len = g.k_len, a.k_slot = p.slot;
+    a.batch = p.B, a.seq_q = per_seq, a.k_len = g.k_len, a.k_slot = p.slot, a.k_row0 = p.row0;
     a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
     attention(a, s);
     GemmEpilogue res;
@@ -514,9 +505,13 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd, kvd = dims.kv_heads * hd, half = hd / 2;
   const int R5 = B * (nq + 1);
   KvCache kv;
-  kv.layer_stride = (long)B * p.slot * kvd;
-  kv.k = c.take<bf16>((size_t)dims.layers * kv.layer_stride);
-  kv.v = c.take<bf16>((size_t)dims.layers * kv.layer_stride);
+  if (p.pool) {  // continuation plan: the caller's pool is the cache
+    kv.k = p.pool->k, kv.v = p.pool->v, kv.layer_stride = p.pool->layer_stride;
+  } else {
+    kv.layer_stride = (long)B * p.slot * kvd;
+    kv.k = c.take<bf16>((size_t)dims.layers * kv.layer_stride);
+    kv.v = c.take<bf16>((size_t)dims.layers * kv.layer_stride);
+  }
   GenBufs g;
   g.cur_tok = c.take<int>(B), g.gen = c.take<int>(B), g.finished = c.take<int>(B), g.next = c.take<int>(B);
   g.k_len = c.take<int>(B), g.n_active = c.take<int>(1), g.out_tokens = c.take<int>((size_t)B * p.max_new);
@@ -544,7 +539,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
     N1_CUDA(cudaStreamSynchronize(s));
     if (active == 0) break;
     // 2. one decode pass: the token just sampled is row (len + gen - 1) of its sequence
-    gen_rows(p.d_len, p.d_delta, g.gen, 1, 1, B, p.slot, g.dest, g.pos3, g.k_len, s);
+    gen_rows(p.d_len, p.d_delta, g.gen, 1, 1, B, p.slot, p.row0, g.dest, g.pos3, g.k_len, s);
     mrope_table(g.pos3, g.rope, B, half, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
     gather_rows(embed_, g.cur_tok, g.x, B, 1, H, s);
     chunk_pass(g, p, kv, 1, s);
@@ -553,7 +548,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   if (latents) {
     // 3. generate_latents(output_ids, ...) on the cache: the last sampled token has no K/V yet, so the pass covers
     //    [last token, TRAJ x nq]; rows 1..nq of each sequence are the latent plan (internvla_n1.py L327, L345).
-    gen_rows(p.d_len, p.d_delta, g.gen, 1, nq + 1, B, p.slot, g.dest, g.pos3, g.k_len, s);
+    gen_rows(p.d_len, p.d_delta, g.gen, 1, nq + 1, B, p.slot, p.row0, g.dest, g.pos3, g.k_len, s);
     mrope_table(g.pos3, g.rope, R5, half, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
     latent_src(g.cur_tok, B, nq, g.kind, g.src, s);
     build_embeds(g.kind, g.src, embed_, nullptr, latentq_, g.x, R5, H, s);
@@ -576,12 +571,34 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
                            int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const {
   N1_CHECK(loaded_ && ws, "llm_generate: not loaded / null workspace");
   N1_CHECK(p.max_new > 0, "llm_generate: the plan was not created for generation");
+  N1_CHECK(!p.pool, "llm_generate: a continuation plan needs its K/V pool (n1_llm_generate_pool)");
   if (!has_lm_head()) throw Error(-6, "llm_generate: lm_head.weight was not part of the loaded state_dict");
   N1_CHECK(out.tokens && out.lens, "llm_generate: null output buffers");
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate: workspace too small");
   p.wait_ready(s);
   gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s);
   p.mark_used(s);
+}
+
+void S2Model::llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
+                                const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents,
+                                cudaStream_t s) const {
+  N1_CHECK(loaded_ && ws, "llm_generate_pool: not loaded / null workspace");
+  N1_CHECK(p.pool == &pool, "llm_generate_pool: the plan was not created for this K/V pool");
+  if (!has_lm_head()) throw Error(-6, "llm_generate_pool: lm_head.weight was not part of the loaded state_dict");
+  N1_CHECK(out.tokens && out.lens, "llm_generate_pool: null output buffers");
+  for (int b = 0; b < p.B; ++b)
+    N1_CHECK(p.h_ctx[b] <= pool.valid[p.h_slot[b]],
+             "llm_generate_pool: sequence " + std::to_string(b) + " reuses " + std::to_string(p.h_ctx[b]) +
+                 " rows but slot " + std::to_string(p.h_slot[b]) + " holds " + std::to_string(pool.valid[p.h_slot[b]]));
+  if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate_pool: workspace too small");
+  for (int b = 0; b < p.B; ++b) pool.valid[p.h_slot[b]] = p.h_ctx[b];  // rows past ctx are rewritten from here on
+  p.wait_ready(s);
+  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s);
+  p.mark_used(s);
+  // K/V exist for the prompt and every generated token but the last; the latent pass writes the last one too (and the
+  // TRAJ rows after it, which are not part of the conversation)
+  for (int b = 0; b < p.B; ++b) pool.valid[p.h_slot[b]] = p.h_len[b] + out.lens[b] - (latents ? 0 : 1);
 }
 
 }  // namespace n1

@@ -31,6 +31,19 @@ struct VitPlan {
   ~VitPlan();
 };
 
+// Caller-owned K/V cache pool: `slots` conversations of up to `cap` rows each, per decoder layer.  Sized once
+// (n1_kv_pool_create) and never reallocated by a hot call.  valid[s] = rows of slot s whose K/V a pass actually wrote
+// for the conversation's tokens (prompt + generated; never the TRAJ rows of the latent pass).
+struct KvPool {
+  bf16 *k = nullptr, *v = nullptr;  // [layers][slots * cap][kv_heads * head_dim]
+  int slots = 0, cap = 0;
+  long layer_stride = 0;
+  std::vector<int> valid;
+  size_t bytes() const { return 2 * (size_t)layer_stride * layers * sizeof(bf16); }
+  int layers = 0;
+  ~KvPool();
+};
+
 // Device-resident token bookkeeping for one batch of prompts (generate_latents appends n_query TRAJ tokens each).
 struct LlmPlan {
   int B = 0, max_len = 0, n_query = 0;
@@ -42,6 +55,12 @@ struct LlmPlan {
   // generation plans only (max_new > 0): every sequence owns `slot` rows of the per-layer K/V cache
   int max_new = 0, slot = 0;
   int *dest_rows = nullptr, *d_len = nullptr, *d_delta = nullptr;  // [tokens], [B], [B]
+  // continuation plans only (pool != nullptr): sequence b reuses the first ctx[b] rows of pool slot h_slot[b]; the plan's
+  // rows are the suffix [ctx[b], len[b]) of each prompt, and its K/V live in the pool (first row row0[b])
+  const KvPool* pool = nullptr;
+  std::vector<int> h_ctx, h_slot, h_len;
+  int *ctx = nullptr, *row0 = nullptr;
+  bool any_ctx = false;  // some sequence reuses rows: the prefill attends through the pool (attention_cache)
   // All device arrays above are carved from ONE pooled block (plan_pool in s2_model.cu): a plan is created every policy
   // step (prompts change), so creation must not cudaMalloc / cudaFree / synchronise once the pool is warm.  `ready` is
   // recorded after the upload + RoPE-table kernel on the creating stream; `last_use` after every hot call, so a recycled
@@ -72,8 +91,13 @@ class S2Model {
   // ids: packed prompt token ids (host), lens[B]; TRAJ tokens are appended per sequence by the planner.
   // max_new_tokens < 0: latent plan (generate_latents).  >= 1: generation plan (no TRAJ tokens; KV-cache slots sized
   // for the prompt + max_new_tokens + n_query rows).
+  // ctx_host / slot_host / pool (all or none; generation plans only): a continuation plan over the FULL prompts and all
+  // their image grids (mRoPE positions come from the whole prompt) that embeds and prefills rows [ctx[b], len[b]) only;
+  // image features are expected for the images whose tokens lie in those rows, and no image may straddle ctx[b].
   LlmPlan* make_llm_plan(const int32_t* ids_host, const int32_t* lens_host, int B, const int32_t* grid_thw_host,
-                         int n_img, cudaStream_t s, int max_new_tokens = -1) const;
+                         int n_img, cudaStream_t s, int max_new_tokens = -1, const int32_t* ctx_host = nullptr,
+                         const int32_t* slot_host = nullptr, const KvPool* pool = nullptr) const;
+  KvPool* make_pool(int slots, int cap) const;
 
   size_t ws_vit(const VitPlan& p) const;
   // pixels bf16 [n_patches, 3 * tpatch * patch^2] -> out bf16 [n_patches / merge^2, v_out] (original token order)
@@ -89,6 +113,9 @@ class S2Model {
   size_t ws_generate(const LlmPlan& p) const;
   void llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, const int32_t* eos, int n_eos,
                     int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const;
+  // the same on a continuation plan: K/V are read from and written to `pool` (the plan's), and pool.valid is updated
+  void llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
+                         const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const;
   bool has_lm_head() const { return lm_head_.w != nullptr; }
 
   // ---- training branch, System-2 half (s2_train.cu)

@@ -123,4 +123,102 @@ void rope_index_one(const int32_t* ids, int len, const int32_t* grid_thw, int n_
   delta = mx + 1 - len;
 }
 
+void plan_rows(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img, const PlanArgs& a,
+               PlanRows& o) {
+  o = PlanRows();
+  const bool cont = a.ctx != nullptr, gen = a.max_new > 0;
+  N1_CHECK(cont == (a.slots != nullptr), "continuation plan: ctx and slots go together");
+  N1_CHECK(!cont || gen, "continuation plan: only generation plans continue a cache");
+  const int nq = gen ? 0 : a.n_query, unit = a.merge * a.merge;
+  if (cont) {
+    std::vector<char> used(a.pool_slots, 0);
+    for (int b = 0; b < B; ++b) {
+      N1_CHECK(a.slots[b] >= 0 && a.slots[b] < a.pool_slots, "continuation plan: slot " + std::to_string(a.slots[b]) +
+                                                                 " out of range [0, " + std::to_string(a.pool_slots) + ")");
+      N1_CHECK(!used[a.slots[b]], "continuation plan: slot " + std::to_string(a.slots[b]) + " used twice in one batch");
+      used[a.slots[b]] = 1;
+      N1_CHECK(a.ctx[b] >= 0 && a.ctx[b] < lens[b], "continuation plan: reused length must be in [0, prompt length)");
+      N1_CHECK((long)lens[b] + a.max_new + a.n_query <= a.pool_cap,
+               "continuation plan: prompt + max_new_tokens + n_query exceeds the pool's slot capacity (" +
+                   std::to_string(a.pool_cap) + ")");
+      o.ctx.push_back(a.ctx[b]), o.slot_of.push_back(a.slots[b]);
+      o.any_ctx |= a.ctx[b] > 0;
+    }
+  }
+  o.cu.push_back(0);
+  int cursor = 0;
+  long off = 0, expect_cont = 0;
+  std::vector<std::vector<int>> pos_seq(B);
+  for (int b = 0; b < B; ++b) {
+    const int len = lens[b];
+    N1_CHECK(len > 0, "empty prompt");
+    std::vector<int> seq(ids + off, ids + off + len);
+    off += len;
+    for (int q = 0; q < nq; ++q) seq.push_back(kTrajTokenId);  // internvla_n1.py L327
+    const int L = (int)seq.size();
+    const int c = cont ? a.ctx[b] : 0;
+    const int first_img = cursor;
+    int delta = 0;
+    rope_index_one(seq.data(), L, grid, n_img, a.merge, cursor, pos_seq[b], delta);
+    o.delta.push_back(delta);
+    if (cont) {  // images of this prompt: those wholly before c were prefilled before, none may straddle c
+      int im = first_img;
+      for (int i = 0; i < L; ++i)
+        if (seq[i] == kImageTokenId && (i == 0 || seq[i - 1] != kImageTokenId)) {
+          N1_CHECK(im < cursor, "image placeholder without a grid row");
+          const int n = grid[im * 3] * grid[im * 3 + 1] * grid[im * 3 + 2] / unit;
+          N1_CHECK(!(i < c && c < i + n), "continuation plan: the reused prefix would end inside an image");
+          if (i >= c) expect_cont += n;
+          ++im;
+        }
+    }
+    for (int i = c; i < L; ++i) {
+      if (i >= len) {
+        o.kind.push_back(2), o.src.push_back(i - len);  // latent_queries[q]
+        o.out_rows.push_back((int)o.kind.size() - 1);
+      } else if (seq[i] == kImageTokenId) {
+        o.kind.push_back(1), o.src.push_back((int)o.n_image_tokens++);  // image features in order (L332)
+      } else {
+        N1_CHECK(seq[i] >= 0 && seq[i] < a.vocab, "token id out of vocabulary");
+        o.kind.push_back(0), o.src.push_back(seq[i]);
+      }
+    }
+    if (gen) o.out_rows.push_back((int)o.kind.size() - 1);  // logits of the last prompt token start the decode
+    o.cu.push_back(o.cu.back() + L - c);
+    o.max_len = std::max(o.max_len, L - c);
+    if (c > 0) {  // keep the positions of rows [c, L) ([3, L - c])
+      std::vector<int> t((size_t)3 * (L - c));
+      for (int st = 0; st < 3; ++st)
+        std::copy(pos_seq[b].begin() + (size_t)st * L + c, pos_seq[b].begin() + (size_t)(st + 1) * L,
+                  t.begin() + (size_t)st * (L - c));
+      pos_seq[b].swap(t);
+    }
+  }
+  const long tokens = o.cu.back();
+  long expect = 0;
+  for (int i = 0; i < cursor; ++i) expect += (long)grid[i * 3] * grid[i * 3 + 1] * grid[i * 3 + 2] / unit;
+  if (cont) expect = expect_cont;
+  N1_CHECK(expect == o.n_image_tokens, "Image features and image tokens do not match: tokens " +
+                                           std::to_string(o.n_image_tokens) + ", features " +
+                                           std::to_string(expect));  // same check as internvla_n1.py L135-138
+  // [3, tokens] layout over the packed batch
+  o.pos3.assign((size_t)3 * tokens, 0);
+  for (int b = 0; b < B; ++b) {
+    const int L = o.cu[b + 1] - o.cu[b];
+    for (int st = 0; st < 3; ++st)
+      for (int i = 0; i < L; ++i) o.pos3[(size_t)st * tokens + o.cu[b] + i] = pos_seq[b][(size_t)st * L + i];
+  }
+  if (gen) {
+    o.slot = cont ? a.pool_cap : o.max_len + a.max_new + a.n_query;
+    o.dest.resize(tokens), o.len.resize(B);
+    for (int b = 0; b < B; ++b) {
+      const int n = o.cu[b + 1] - o.cu[b], c = cont ? a.ctx[b] : 0;
+      const int r0 = cont ? a.slots[b] * a.pool_cap : b * o.slot;
+      o.len[b] = c + n;
+      for (int i = 0; i < n; ++i) o.dest[o.cu[b] + i] = r0 + c + i;
+      if (cont) o.row0.push_back(r0);
+    }
+  }
+}
+
 }  // namespace n1

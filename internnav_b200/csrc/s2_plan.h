@@ -32,4 +32,31 @@ void vit_index(const int32_t* grid_thw, int n_img, int merge, int vit_merger_win
 void rope_index_one(const int32_t* ids, int len, const int32_t* grid_thw, int n_img, int merge, int& cursor,
                     std::vector<int>& pos3, int& delta);
 
+// Token bookkeeping of one decoder plan over B packed prompts (all host integer work of S2Model::make_llm_plan).
+//   max_new < 0: latent plan (n_query TRAJ tokens appended per prompt); >= 1: generation plan, K/V rows of sequence b at
+//   b * slot + i with slot = max_len + max_new + n_query.
+//   ctx / slots (continuation plan, generation only): sequence b reuses the first ctx[b] rows of pool slot slots[b]
+//   (pool_slots x pool_cap rows); its rows are [ctx[b], len[b]) only, their K/V rows slots[b] * pool_cap + i, and image
+//   features are expected for the images after ctx[b] alone.
+struct PlanArgs {
+  int merge = 2, vocab = 0, n_query = 0, max_new = -1;
+  const int32_t* ctx = nullptr;
+  const int32_t* slots = nullptr;
+  int pool_slots = 0, pool_cap = 0;
+};
+struct PlanRows {
+  std::vector<int> cu;                  // [B + 1] planned rows per sequence, packed
+  std::vector<int> kind, src;           // [rows] 0 text (src = token id), 1 image (src = feature row), 2 latent query
+  std::vector<int> out_rows;            // rows read after the last layer
+  std::vector<int> pos3;                // [3, rows] mRoPE positions
+  std::vector<int> delta;               // [B] mRoPE delta
+  std::vector<int> dest, len;           // generation plans: [rows] K/V cache row, [B] keys after the prefill (= prompt length)
+  std::vector<int> ctx, slot_of, row0;  // continuation plans: [B] reused rows, pool slot, first K/V row of the slot
+  long n_image_tokens = 0;
+  int max_len = 0, slot = 0;
+  bool any_ctx = false;
+};
+void plan_rows(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img, const PlanArgs& a,
+               PlanRows& o);
+
 }  // namespace n1

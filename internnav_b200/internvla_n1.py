@@ -177,7 +177,12 @@ class InternVLAN1ForCausalLM:
         return_dict_in_generate=True).sequences` (internvla_n1_policy.py L169-176) for B prompts.  `sequences` is
         [B, S_max + longest generation] int64: prompt, generated ids (the eos id included), then `pad_token_id`; ragged
         prompts are right-aligned the way the HF processor pads them (left padding).  Other HF keyword arguments
-        (attention_mask, use_cache, past_key_values, ...) are accepted and have no effect on greedy search."""
+        (attention_mask, use_cache, ...) are accepted and have no effect on greedy search.  `past_key_values`: one KVCache
+        (or None) per prompt, from `make_kv_pool(...).handle(slot)` or a previous call's `out.past_key_values`; the
+        longest reusable prefix of each prompt is then neither re-encoded nor re-prefilled (qwen.System2._generate_cached),
+        and the output also carries `past_key_values` (one new KVCache per prompt), `prefill_rows` and `vit_patches`.
+        A None entry next to KVCaches starts a fresh conversation on an unused slot of their pool; a list of None only
+        (no pool to write to) is an uncached call."""
         if do_sample or hf_kwargs.get("num_beams", 1) != 1:
             raise NotImplementedError("n1b200 implements greedy search only (the reference calls do_sample=False)")
         eos = EOS_TOKEN_IDS if eos_token_id is None else \
@@ -185,9 +190,13 @@ class InternVLAN1ForCausalLM:
         pad = PAD_TOKEN_ID if pad_token_id is None else int(pad_token_id)
         prompts = self._prompts(input_ids)
         grid = image_grid_thw.tolist() if torch.is_tensor(image_grid_thw) else image_grid_thw
+        caches = hf_kwargs.get("past_key_values")
+        if caches is not None and all(c is None for c in caches):
+            caches = None
+        extra = {} if caches is None else {"past_key_values": caches}
         with torch.no_grad():
             toks, lat, passes = self._s2.generate(prompts, pixel_values, grid, max_new_tokens=int(max_new_tokens),
-                                                  eos_token_ids=eos, pad_token_id=pad, with_latents=with_latents)
+                                                  eos_token_ids=eos, pad_token_id=pad, with_latents=with_latents, **extra)
         s_max = max(len(p) for p in prompts)
         g_max = max(len(t) for t in toks)
         seq = torch.full((len(prompts), s_max + g_max), pad, dtype=torch.int64)
@@ -195,7 +204,16 @@ class InternVLAN1ForCausalLM:
             seq[b, s_max - len(p):s_max] = torch.tensor(p, dtype=torch.int64)
             seq[b, s_max:s_max + len(t)] = torch.tensor(t, dtype=torch.int64)
         out = SimpleNamespace(sequences=seq.to(self.device), generated=toks, latents=lat, decode_passes=passes)
+        if caches is not None:  # one KVCache per prompt (None: the conversation did not fit its slot)
+            info = self._s2.last_cache
+            out.past_key_values, out.prefill_rows, out.vit_patches = info["caches"], info["prefill_rows"], info["vit_patches"]
         return out if (return_dict_in_generate or with_latents) else out.sequences
+
+    def make_kv_pool(self, slots, capacity):
+        """A K/V cache pool for `slots` conversations of up to `capacity` tokens (prompt + generated + n_query rows),
+        allocated once: 2 * layers * kv_heads * head_dim * 2 bytes per token and slot."""
+        from .qwen import KVPool
+        return KVPool(self._s2, slots, capacity)
 
     def generate_with_latents(self, input_ids, pixel_values, image_grid_thw, max_new_tokens=128, **kw):
         """One System-2 call of the dual-system policy (internvla_n1_policy.py L166-195): greedy answer tokens AND the

@@ -13,6 +13,7 @@ available offline.  Anything with `apply_chat_template`, `__call__(text=[...], i
 """
 import copy
 import itertools
+import math
 import re
 from collections import OrderedDict
 from types import SimpleNamespace
@@ -75,6 +76,10 @@ class InternVLAN1Policy:
         self.max_new_tokens = max_new_tokens
         self.device = device if device is not None else getattr(model, "device", "cpu")
         self.episodes = [_Episode() for _ in range(num_envs)]
+        # K/V cache of each environment's last System-2 conversation, passed back on its look-down turn only (the turn
+        # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
+        self._kv_pool = None
+        self._kv = [None] * num_envs
 
     def eval(self):
         return self
@@ -82,6 +87,27 @@ class InternVLAN1Policy:
     def reset(self, env_ids=None):
         for e in (range(len(self.episodes)) if env_ids is None else env_ids):
             self.episodes[e] = _Episode()
+            self._kv[e] = None
+
+    def _kv_capacity(self, frame_h, frame_w):
+        """Tokens one environment's slot must hold: a fresh turn (num_history + 1 resized frames), the look-down frame at
+        full size, two answers, the TRAJ rows, and 512 tokens for the text of both turns.  A conversation that still
+        does not fit runs uncached."""
+        def img(h, w):
+            return math.ceil(h / 28) * math.ceil(w / 28)
+        nq = getattr(getattr(self.model, "config", None), "n_query", 4)
+        return ((self.num_history + 1) * img(self.resize_h, self.resize_w) + img(frame_h, frame_w) +
+                2 * self.max_new_tokens + nq + 512)
+
+    def _caches(self, env_ids, look_downs, frame):
+        """past_key_values for one call, or None when the model keeps no K/V caches."""
+        make = getattr(self.model, "make_kv_pool", None)
+        if make is None:
+            return None
+        if self._kv_pool is None:
+            self._kv_pool = make(len(self.episodes), self._kv_capacity(*frame.shape[:2]))
+        return [self._kv[e] if ld and self._kv[e] is not None else self._kv_pool.handle(e)
+                for e, ld in zip(env_ids, look_downs)]
 
     def step_no_infer(self, env_ids, rgbs, depths=None, poses=None):
         for e, rgb in zip(env_ids, rgbs):
@@ -140,9 +166,16 @@ class InternVLAN1Policy:
         prompts = [inp["input_ids"][0].tolist() for _, inp in prepared]
         pixels = torch.cat([inp["pixel_values"] for _, inp in prepared], dim=0)
         grids = torch.cat([torch.stack(list(inp["image_grid_thw"])).reshape(-1, 3) for _, inp in prepared], dim=0)
+        caches = self._caches([env_ids[j] for j, _ in prepared], [look_downs[j] for j, _ in prepared], rgbs[prepared[0][0]])
         with torch.no_grad():
-            out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens)
+            if caches is None:
+                out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens)
+            else:
+                out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens,
+                                                       past_key_values=caches)
         for n, (j, _) in enumerate(prepared):
+            if caches is not None:
+                self._kv[env_ids[j]] = out.past_key_values[n]
             ep = self.episodes[env_ids[j]]
             ep.llm_output = self.processor.tokenizer.decode(out.generated[n], skip_special_tokens=True)
             res = S2Output()

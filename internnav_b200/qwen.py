@@ -5,6 +5,7 @@ equivalents of the calls InternVLAN1ForCausalLM.generate_latents makes (internvl
 `visual(pixel_values, grid_thw)` and `model(inputs_embeds, position_ids)` + the last-n_query slice.
 """
 import ctypes
+import itertools
 
 import torch
 
@@ -93,6 +94,32 @@ def _bind(L):
     L.n1_s2_train_forward.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
     L.n1_s2_train_backward.restype = ctypes.c_int
     L.n1_s2_train_backward.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
+    L.n1_kv_pool_create.restype = ctypes.c_int
+    L.n1_kv_pool_create.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]
+    L.n1_kv_pool_destroy.restype = None
+    L.n1_kv_pool_destroy.argtypes = [vp]
+    L.n1_kv_pool_bytes.restype = ctypes.c_size_t
+    L.n1_kv_pool_bytes.argtypes = [vp]
+    L.n1_kv_pool_valid.restype = ctypes.c_int
+    L.n1_kv_pool_valid.argtypes = [vp, ctypes.c_int]
+    L.n1_kv_pool_read.restype = ctypes.c_int
+    L.n1_kv_pool_read.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp]
+    i32p = ctypes.POINTER(ctypes.c_int32)
+    L.n1_plan_rows_host.restype = ctypes.c_int
+    L.n1_plan_rows_host.argtypes = [i32p, i32p, ctypes.c_int, i32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, i32p, i32p, ctypes.c_int, i32p, i32p, i32p,
+                                    i32p, i32p, i32p]
+    L.n1_gen_plan_create_cont.restype = ctypes.c_int
+    L.n1_gen_plan_create_cont.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
+                                          ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.c_int, vp,
+                                          ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(vp),
+                                          vp]
+    L.n1_llm_generate_pool.restype = ctypes.c_int
+    L.n1_llm_generate_pool.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp, ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
+                                       ctypes.c_int32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
+                                       ctypes.POINTER(ctypes.c_int32), vp]
+    L.n1_image_digest.restype = ctypes.c_int
+    L.n1_image_digest.argtypes = [vp, ctypes.c_int64, vp, ctypes.c_int, vp, vp]
     L._s2_bound = True
 
 
@@ -100,7 +127,9 @@ S2_SYMBOLS = ["n1_s2_load", "n1_vit_plan_create", "n1_vit_plan_destroy", "n1_vit
               "n1_llm_plan_destroy", "n1_llm_plan_tokens", "n1_llm_plan_image_tokens", "n1_llm_plan_positions",
               "n1_vit_workspace_bytes", "n1_llm_workspace_bytes", "n1_qwen_vit", "n1_llm_prefill", "n1_rope_index",
               "n1_vit_window_index", "n1_gen_plan_create", "n1_generate_workspace_bytes", "n1_s2_has_lm_head",
-              "n1_llm_generate", "n1_s2_train_workspace_bytes", "n1_s2_train_forward", "n1_s2_train_backward", "n1_s2_set_latent_queries"]
+              "n1_llm_generate", "n1_s2_train_workspace_bytes", "n1_s2_train_forward", "n1_s2_train_backward", "n1_s2_set_latent_queries",
+              "n1_kv_pool_create", "n1_kv_pool_destroy", "n1_kv_pool_bytes", "n1_kv_pool_valid", "n1_kv_pool_read", "n1_plan_rows_host", "n1_gen_plan_create_cont",
+              "n1_llm_generate_pool", "n1_image_digest"]
 
 EOS_TOKEN_IDS = (151645, 151643)  # Qwen2.5-VL generation_config.json: <|im_end|>, <|endoftext|>
 PAD_TOKEN_ID = 151643
@@ -120,6 +149,105 @@ def normalise_keys(state_dict):
         if k.startswith("visual.") or k.startswith("model.") or k == "lm_head.weight":
             out[k] = v
     return out
+
+
+IMAGE_TOKEN_ID = 151655
+
+
+def image_spans(prompt, grids, merge=2):
+    """(first token, token count) of every image of a prompt, in order; `grids` are the prompt's image grids."""
+    spans, i, k = [], 0, 0
+    while i < len(prompt):
+        if prompt[i] == IMAGE_TOKEN_ID:
+            t, h, w = (int(v) for v in grids[k])
+            n = t * h * w // (merge * merge)
+            spans.append((i, n))
+            i, k = i + n, k + 1
+        else:
+            i += 1
+    return spans
+
+
+def reuse_length(handle_tokens, handle_images, prompt, images, cap, need):
+    """Rows of a cached conversation a new prompt may reuse: the longest common token prefix, cut
+      * at the first image of the prompt whose content digest differs from the cached one at the same position (every
+        image token has the same id, so only the digest tells two images apart),
+      * at the first image the prefix would split,
+      * below the prompt length (the last prompt row must be prefilled: its logits start the decode).
+    handle_tokens: ids the cache holds K/V for; handle_images / images: {first token: (count, digest)} and [(first token,
+    count, digest)].  0 when the conversation does not fit the slot (`need` rows > `cap`)."""
+    if need > cap:
+        return 0
+    n = 0
+    m = min(len(handle_tokens), len(prompt) - 1)
+    while n < m and handle_tokens[n] == prompt[n]:
+        n += 1
+    for st, cnt, dg in images:
+        if st >= n:
+            break
+        if st + cnt > n or handle_images.get(st) != (cnt, dg):
+            return st
+    return n
+
+
+class KVCache:
+    """One conversation's K/V in a slot of a KVPool (HF's `past_key_values` for one prompt): the token ids it covers and
+    the position, length and content digest of each image among them.  A handle is stale once its slot is rewritten."""
+
+    def __init__(self, pool, slot, tokens=(), images=None, version=None):
+        self.pool, self.slot = pool, int(slot)
+        self.tokens = list(tokens)
+        self.images = dict(images or {})
+        self.version = pool.version[self.slot] if version is None else version
+
+    def __len__(self):
+        return len(self.tokens) if self.version == self.pool.version[self.slot] else 0
+
+
+class KVPool:
+    """Caller-owned device memory for `slots` conversations of up to `capacity` tokens, sized once."""
+    _serials = itertools.count()
+
+    def __init__(self, s2, slots, capacity):
+        L = _lib.lib()
+        _bind(L)
+        self.s2, self.slots, self.capacity = s2, int(slots), int(capacity)
+        h = c_void_p()
+        with torch.cuda.device(s2.device):
+            check(L.n1_kv_pool_create(s2._h(), self.slots, self.capacity, ctypes.byref(h)))
+        self._p = h
+        self.serial = next(KVPool._serials)  # identifies the pool in System2's plan cache (ids and addresses are reused)
+        self.version = [0] * self.slots
+
+    @property
+    def bytes(self):
+        return int(_lib.lib().n1_kv_pool_bytes(self._p))
+
+    def valid(self, slot):
+        r = _lib.lib().n1_kv_pool_valid(self._p, int(slot))
+        if r < 0:
+            check(r)
+        return r
+
+    def read(self, layer, slot, row, n):
+        """(K, V) rows [row, row + n) of `slot` in decoder layer `layer`: bf16 [n, kv_heads * head_dim] copies."""
+        w = self.s2.cfg["kv_heads"] * self.s2.cfg["head_dim"]
+        k = torch.empty(n, w, device=self.s2.device, dtype=torch.bfloat16)
+        v = torch.empty_like(k)
+        check(_lib.lib().n1_kv_pool_read(self._p, int(layer), int(slot), int(row), int(n), _lib.ptr(k), _lib.ptr(v),
+                                         _lib.stream_ptr()))
+        return k, v
+
+    def handle(self, slot):
+        """An empty cache on `slot`: passing it to generate() writes the conversation there."""
+        return KVCache(self, slot)
+
+    def __del__(self):
+        try:
+            if self._p:
+                _lib.lib().n1_kv_pool_destroy(self._p)
+        except Exception:
+            pass
 
 
 class System2:
@@ -315,11 +443,15 @@ class System2:
         return hit[0]
 
     def generate(self, prompts, pixel_values, grid_thw, max_new_tokens=128, eos_token_ids=EOS_TOKEN_IDS,
-                 pad_token_id=PAD_TOKEN_ID, with_latents=False, image_feats=None):
+                 pad_token_id=PAD_TOKEN_ID, with_latents=False, image_feats=None, past_key_values=None):
         """Greedy decode for B prompts (`model.generate(do_sample=False, max_new_tokens=...)`, internvla_n1_policy.py
         L169-176).  Returns (list of B generated-token lists, each ending with its eos id unless the budget ran out,
         latents [B, n_query, hidden] or None, decode passes run).  With `with_latents` the K/V cache of the decode is
-        extended by the TRAJ tokens, which equals `generate_latents(output_ids, ...)` without a second prefill."""
+        extended by the TRAJ tokens, which equals `generate_latents(output_ids, ...)` without a second prefill.
+        `past_key_values`: one KVCache per prompt (see _generate_cached); the call then also sets `self.last_cache`."""
+        if past_key_values is not None:
+            return self._generate_cached(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
+                                         with_latents, past_key_values)
         L = _lib.lib()
         if not L.n1_s2_has_lm_head(self._h()):
             raise RuntimeError("generate() needs lm_head.weight in the loaded state_dict; there is no fallback")
@@ -340,3 +472,112 @@ class System2:
                                 int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
         out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
         return out, lat, passes.value
+
+    def image_digests(self, px, grid_thw):
+        """Content digest (uint64 as int64) of every image of device bf16 pixel rows `px`, computed on the device."""
+        sizes = [int(t) * int(h) * int(w) for t, h, w in grid_thw]
+        off = torch.tensor([0] + sizes, dtype=torch.int64).cumsum(0).to(self.device)
+        out = torch.empty(len(sizes), dtype=torch.int64, device=self.device)
+        check(_lib.lib().n1_image_digest(_lib.ptr(px), px.shape[1], _lib.ptr(off), len(sizes), _lib.ptr(out),
+                                         _lib.stream_ptr()))
+        return out.tolist()
+
+    def _generate_cached(self, prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id, with_latents,
+                         caches):
+        """generate() continuing cached conversations.  caches[b] is a KVCache of one KVPool (an empty one for a fresh
+        prompt; all slots distinct) or None: a fresh conversation on a slot no other entry uses (one never written if
+        there is one, else the lowest; a cache held elsewhere on that slot goes stale).  Prompt b reuses reuse_length(...) rows of its slot: only the images after that
+        prefix go through the vision tower and only the rows after it are prefilled.  Afterwards the slot holds the new
+        conversation and `self.last_cache` = dict(caches=[one new KVCache per prompt], prefill_rows, vit_patches, reused).
+        A batch in which some conversation does not fit its slot runs as an uncached call and returns no caches."""
+        L = _lib.lib()
+        B = len(prompts)
+        if len(caches) != B or all(c is None for c in caches):
+            raise ValueError("past_key_values: one KVCache or None per prompt, at least one KVCache")
+        pool = next(c for c in caches if c is not None).pool
+        given = [c for c in caches if c is not None]
+        if any(c.pool is not pool for c in given) or len({c.slot for c in given}) != len(given):
+            raise ValueError("past_key_values: the caches of one call must be distinct slots of one KVPool")
+        # a None entry starts a fresh conversation on a slot no other entry uses: one never written first, then the lowest
+        free = sorted((s_ for s_ in range(pool.slots) if s_ not in {c.slot for c in given}),
+                      key=lambda s_: (pool.valid(s_) > 0, s_))
+        if len(free) < B - len(given):
+            raise ValueError("past_key_values: the pool has no free slot for a None entry")
+        free = iter(free)
+        caches = [c if c is not None else pool.handle(next(free)) for c in caches]
+        nq, merge = self.cfg["n_query"], self.cfg["v_merge"]
+        need = [len(p) + int(max_new_tokens) + nq for p in prompts]
+        if any(n > pool.capacity for n in need):
+            toks, lat, passes = self.generate(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
+                                              with_latents)
+            n_p = sum(int(t) * int(h) * int(w) for t, h, w in grid_thw)
+            self.last_cache = dict(caches=[None] * B, prefill_rows=sum(len(p) for p in prompts), vit_patches=n_p,
+                                   reused=[0] * B)
+            return toks, lat, passes
+        px = pixel_values.to(self.device, torch.bfloat16).contiguous()
+        digests = self.image_digests(px, grid_thw)
+        reused, keep_rows, keep_grids, images = [], [], [], []
+        gi, row = 0, 0
+        for b, (p, c) in enumerate(zip(prompts, caches)):
+            spans = image_spans(p, grid_thw[gi:], merge)
+            imgs = [(st, n, digests[gi + k]) for k, (st, n) in enumerate(spans)]
+            r = reuse_length(c.tokens, c.images, p, imgs, pool.capacity, need[b]) if len(c) else 0
+            r = min(r, pool.valid(c.slot)) if r else 0
+            for k, (st, n, dg) in enumerate(imgs):  # patch rows of the images after the reused prefix
+                t, h, w = (int(v) for v in grid_thw[gi + k])
+                if st >= r:
+                    keep_rows.append((row, row + t * h * w))
+                    keep_grids.append(grid_thw[gi + k])
+                row += t * h * w
+            reused.append(r)
+            images.append({st: (n, dg) for st, n, dg in imgs})
+            gi += len(spans)
+        if keep_rows:
+            sub = px if len(keep_rows) == len(grid_thw) else torch.cat([px[a:e] for a, e in keep_rows])
+            feats = self.visual(sub, keep_grids)
+        else:
+            feats = torch.empty(0, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16)
+        slots = [c.slot for c in caches]
+        plan = self._cont_plan(prompts, grid_thw, max_new_tokens, pool, reused, slots)
+        assert feats.shape[0] == L.n1_llm_plan_image_tokens(plan), "image features and image tokens do not match"
+        lat = torch.empty(B, nq, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) if with_latents else None
+        nb = L.n1_generate_workspace_bytes(self._h(), plan)
+        ws = self._scratch("gen", nb)
+        eos = (ctypes.c_int32 * max(1, len(eos_token_ids)))(*[int(e) for e in eos_token_ids])
+        toks = (ctypes.c_int32 * (B * int(max_new_tokens)))()
+        lens = (ctypes.c_int32 * B)()
+        passes = ctypes.c_int32(0)
+        for s_ in slots:  # the call rewrites these slots: every older handle on them is stale from here on
+            pool.version[s_] += 1
+        check(L.n1_llm_generate_pool(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), eos,
+                                     len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
+                                     ctypes.byref(passes), _lib.stream_ptr()))
+        out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
+        new = []
+        for b, p in enumerate(prompts):
+            valid = pool.valid(slots[b])
+            new.append(KVCache(pool, slots[b], (p + out[b])[:valid], images[b]))
+        self.last_cache = dict(caches=new, prefill_rows=int(L.n1_llm_plan_tokens(plan)),
+                               vit_patches=sum(e - a for a, e in keep_rows), reused=reused)
+        return out, lat, passes.value
+
+    def _cont_plan(self, prompts, grid_thw, max_new_tokens, pool, reused, slots):
+        gkey = tuple(int(v) for g in grid_thw for v in g)
+        key = ("cont", pool.serial, int(max_new_tokens), tuple(tuple(p) for p in prompts), gkey, tuple(reused), tuple(slots))
+        hit = self._llm_plans.get(key)
+        if hit is None:
+            L = _lib.lib()
+            flat = [int(t) for p in prompts for t in p]
+            ids = (ctypes.c_int32 * len(flat))(*flat)
+            lens = (ctypes.c_int32 * len(prompts))(*[len(p) for p in prompts])
+            garr = (ctypes.c_int32 * max(1, len(gkey)))(*gkey)
+            ctx = (ctypes.c_int32 * len(prompts))(*reused)
+            sl = (ctypes.c_int32 * len(prompts))(*slots)
+            p = c_void_p()
+            with torch.cuda.device(self.device):
+                check(L.n1_gen_plan_create_cont(self._h(), ids, lens, len(prompts), garr, len(gkey) // 3,
+                                                int(max_new_tokens), pool._p, ctx, sl, ctypes.byref(p), _lib.stream_ptr()))
+            self._evict_plans(L)
+            hit = (p, len(prompts))
+            self._llm_plans[key] = hit
+        return hit[0]
