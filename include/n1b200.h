@@ -261,6 +261,25 @@ int n1_resize_f32(n1_resize_plan p, const void* src_f32, int n_frames, float mul
 int n1_resize_coeffs(int in_size, int out_size, int capacity_k, int32_t* bounds_host, double* weights_host,
                      int32_t* fixed_host, int32_t* ksize);
 
+/* ------------------------------------------------------------------------------------------------ System-2 image rows
+ * replaces: the rescale, normalise and patchify of the Qwen2-VL image processor, per image on the host in the reference
+ * (`processor(text, images)` in internvla_n1_policy.py L164; Qwen2VLImageProcessor with patch 14, temporal patch 2,
+ * merge 2).  The frames are already resized with Pillow's bicubic to a multiple of 28 (n1_resize_rgb_u8, dst_u8).
+ * Rescale + normalise of a uint8 pixel is lut_bf16[c * 256 + byte] ([3, 256], built by the caller with the processor's
+ * own arithmetic), so the rows are bit-equal to the processor's float32 rows converted to bf16.
+ * out_bf16 [n_rows, 1176] (16-byte aligned): image i fills rows [row0, row0 + h * w / 196) in the processor's order
+ * (merged 2 x 2 blocks row-major, their 4 patches row-major; element c * 392 + t * 196 + py * 14 + px, the two t equal).
+ * images_host [n_img] are in output order: row0 of each image is the rows of the images before it, and n_rows their
+ * sum.  ws: n1_vl_patchify_workspace_bytes(n_img).  One launch. */
+typedef struct {
+  const void* src_u8; /* resized frame uint8 [h, w, 3], DEVICE */
+  int32_t h, w;       /* multiples of 28 */
+  int64_t row0;
+} n1_vl_image;
+size_t n1_vl_patchify_workspace_bytes(int n_img);
+int n1_vl_patchify(const n1_vl_image* images_host, int n_img, const void* lut_bf16, void* out_bf16, int64_t n_rows,
+                   void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ training: backward primitives
  * First version of the backward kernels of the training branch (internvla_n1.py L58-318; navdp.py L291-312), exposed
  * one primitive at a time for parity tests against oracle/navdp_backward.py / oracle/qwen_backward.py.

@@ -483,6 +483,18 @@ int n1_resize_coeffs(int in_size, int out_size, int capacity_k, int32_t* bounds,
   });
 }
 
+static_assert(sizeof(n1_vl_image) == sizeof(VlImage) && offsetof(n1_vl_image, row0) == offsetof(VlImage, row0),
+              "n1_vl_image and VlImage must share one layout");
+size_t n1_vl_patchify_workspace_bytes(int n_img) { return vl_patchify_workspace_bytes(n_img); }
+int n1_vl_patchify(const n1_vl_image* images, int n_img, const void* lut, void* out, int64_t n_rows, void* ws,
+                   size_t ws_bytes, void* stream) {
+  return guard([&] {
+    if (!images || !lut || !out || !ws) throw Error(N1_ERR_ARG, "n1_vl_patchify: null arguments");
+    if (ws_bytes < vl_patchify_workspace_bytes(n_img)) throw Error(N1_ERR_WORKSPACE, "n1_vl_patchify: workspace too small");
+    vl_patchify(reinterpret_cast<const VlImage*>(images), n_img, B16(lut), B16(out), n_rows, ws, S(stream));
+  });
+}
+
 size_t n1_rgb_tokens_workspace_bytes(n1_handle h, int B) {
   size_t r = 0;
   guard([&] {

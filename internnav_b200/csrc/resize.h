@@ -38,4 +38,17 @@ void resize_rgb_u8(const ResizePlan& p, const uint8_t* src, int n, float* dst_f3
 void resize_f32(const ResizePlan& p, const float* src, int n, float mul, float clip_max, float* dst, void* ws,
                 cudaStream_t s);
 
+// System-2 image rows (vl_patch.cu).  The Qwen2-VL image processor resizes each image with Pillow to a multiple of 28
+// and then rescales, normalises and patchifies it; after a uint8 resize, rescale + normalise is a per-channel table of
+// the 256 byte values, so the rows are table lookups of the resized frame's bytes.
+struct VlImage {       // layout of n1_vl_image
+  const uint8_t* src;  // resized frame [h, w, 3], device
+  int32_t h, w;        // multiples of 28
+  int64_t row0;        // first output row = rows of the images before it
+};
+size_t vl_patchify_workspace_bytes(int n_img);
+// images HOST [n_img]; lut bf16 [3, 256]; out bf16 [n_rows, 1176] (16-byte aligned), n_rows = sum h * w / 196;
+// ws: vl_patchify_workspace_bytes(n_img) (receives the table)
+void vl_patchify(const VlImage* images, int n_img, const bf16* lut, bf16* out, long n_rows, void* ws, cudaStream_t s);
+
 }  // namespace n1

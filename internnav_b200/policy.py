@@ -10,6 +10,13 @@ The HF processor (chat template + tokenizer + Qwen2-VL image processor) is injec
 collaborator (`AutoProcessor.from_pretrained(model_path)`, L44-47) and needs the checkpoint directory, which is not
 available offline.  Anything with `apply_chat_template`, `__call__(text=[...], images=[...], return_tensors="pt")` and
 `.tokenizer.decode` works (tests use oracle/policy_script.FakeProcessor).
+
+Images take one of two paths.  When the policy runs on a CUDA device and the processor's `image_processor` is one that
+`QwenImagePreprocessor` reproduces (the PIL-backed Qwen2-VL processor), every frame is prepared on the device: the
+history keeps device uint8 frames, the frames of one call are uploaded and resized together, and the pixel rows of all
+environments come from one `QwenImagePreprocessor` call, bit-equal to the processor's.  The processor then only
+tokenises the chat text, with each image placeholder expanded as it would expand it.  Otherwise every frame is a PIL
+image and the processor prepares each environment's prompt on the host, as in the reference.
 """
 import copy
 import itertools
@@ -23,6 +30,7 @@ import torch
 from PIL import Image
 
 from .postprocess import batched_traj_to_actions, chunk_token, s1_action_list
+from .preprocess import QwenImagePreprocessor
 
 DEFAULT_IMAGE_TOKEN = "<image>"
 PROMPT = ("You are an autonomous navigation assistant. Your task is to <instruction>. Where should you go next to stay "
@@ -57,7 +65,8 @@ class S2Output(SimpleNamespace):
 
 
 class _Episode:
-    """Per-environment conversation state (the instance attributes of the reference class, L52-57 / L88-94)."""
+    """Per-environment conversation state (the instance attributes of the reference class, L52-57 / L88-94).  The frames
+    of rgb_list / input_images are PIL images on the host path and device uint8 [H, W, 3] tensors on the device path."""
 
     def __init__(self):
         self.rgb_list = []
@@ -80,6 +89,10 @@ class InternVLAN1Policy:
         # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
         self._kv_pool = None
         self._kv = [None] * num_envs
+        # System-2 images on the device when the processor's image arithmetic can be reproduced there
+        self._vl = None
+        if torch.device(self.device).type == "cuda":
+            self._vl = QwenImagePreprocessor.from_hf(getattr(processor, "image_processor", None), self.device)
 
     def eval(self):
         return self
@@ -110,10 +123,33 @@ class InternVLAN1Policy:
                 for e, ld in zip(env_ids, look_downs)]
 
     def step_no_infer(self, env_ids, rgbs, depths=None, poses=None):
-        for e, rgb in zip(env_ids, rgbs):
+        if self._vl is not None:
+            frames = self._device_frames(rgbs, [True] * len(rgbs))
+        else:
+            frames = [Image.fromarray(rgb).convert("RGB").resize((self.resize_w, self.resize_h)) for rgb in rgbs]
+        for e, frame in zip(env_ids, frames):
             ep = self.episodes[e]
-            ep.rgb_list.append(Image.fromarray(rgb).convert("RGB").resize((self.resize_w, self.resize_h)))
+            ep.rgb_list.append(frame)
             ep.episode_idx += 1
+
+    def _device_frames(self, rgbs, resize):
+        """Raw frames -> device uint8 frames: each uploaded once, those with resize[i] set resized to resize_h x resize_w
+        (Pillow's bicubic), the others kept at full size.  One upload and at most one resize per (shape, resize)."""
+        groups = {}
+        for i, rgb in enumerate(rgbs):
+            a = np.asarray(rgb)
+            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[-1] != 3:
+                a = np.asarray(Image.fromarray(rgb).convert("RGB"))
+            groups.setdefault((a.shape, bool(resize[i])), []).append((i, a))
+        out = [None] * len(rgbs)
+        for (_, rs), members in groups.items():
+            x = torch.from_numpy(np.stack([a for _, a in members])).to(self.device)
+            if rs:
+                x = self._vl.resize(x, (self.resize_h, self.resize_w))
+            # every frame owns its memory, so dropping one environment's history frees it
+            for k, (i, _) in enumerate(members):
+                out[i] = x[k].clone() if len(members) > 1 else x[0]
+        return out
 
     # ------------------------------------------------------------------ System 2
     def _build_inputs(self, ep, rgb, instruction, look_down):
@@ -121,6 +157,13 @@ class InternVLAN1Policy:
         image = Image.fromarray(rgb).convert("RGB")
         if not look_down:
             image = image.resize((self.resize_w, self.resize_h))
+        chat = self._chat(ep, image, instruction, look_down)
+        return self.processor(text=[chat], images=ep.input_images, return_tensors="pt")
+
+    def _chat(self, ep, image, instruction, look_down):
+        """L113-163 for one environment: records the (resized, unless look_down) frame and extends the conversation ->
+        the chat text, one image placeholder per image of ep.input_images."""
+        if not look_down:
             ep.rgb_list.append(image)
             ep.conversation_history = []
             text = PROMPT.replace("<instruction>.", instruction)
@@ -147,25 +190,59 @@ class InternVLAN1Policy:
             else:
                 content.append({"type": "text", "text": part})
         ep.conversation_history.append({"role": "user", "content": content})
-        chat = self.processor.apply_chat_template(ep.conversation_history, tokenize=False, add_generation_prompt=True)
-        return self.processor(text=[chat], images=ep.input_images, return_tensors="pt")
+        return self.processor.apply_chat_template(ep.conversation_history, tokenize=False, add_generation_prompt=True)
+
+    def _expand_image_tokens(self, chat, grids):
+        """Qwen2_5_VLProcessor.__call__'s text expansion: the k-th image placeholder becomes gh * gw / merge^2 of them."""
+        tok = self.processor.image_token
+        parts = chat.split(tok)
+        assert len(parts) == len(grids) + 1, "%d image placeholders for %d images" % (len(parts) - 1, len(grids))
+        merge2 = QwenImagePreprocessor.MERGE ** 2
+        return parts[0] + "".join(tok * (int(t * h * w) // merge2) + p for (t, h, w), p in zip(grids.tolist(), parts[1:]))
+
+    def _prepare_device(self, env_ids, rgbs, instructions, look_downs, results):
+        """The device path of s2_step's input preparation -> (prepared [(j, input_ids list)], device bf16 pixel rows,
+        image_grid_thw); per-environment failures go to results[j]."""
+        frames = self._device_frames(rgbs, [not ld for ld in look_downs])
+        chats = []
+        for j, (e, ins, ld) in enumerate(zip(env_ids, instructions, look_downs)):
+            try:
+                chats.append((j, self._chat(self.episodes[e], frames[j], ins, ld)))
+            except Exception as exc:  # noqa: BLE001 -- reported per environment; the agent applies the retry rule
+                results[j] = exc
+        if not chats:
+            return [], None, None
+        pixels, grids = self._vl([im for j, _ in chats for im in self.episodes[env_ids[j]].input_images])
+        prepared, g = [], 0
+        for j, chat in chats:
+            n = len(self.episodes[env_ids[j]].input_images)
+            text = self._expand_image_tokens(chat, grids[g:g + n])
+            prepared.append((j, self.processor(text=[text], return_tensors="pt")["input_ids"][0].tolist()))
+            g += n
+        return prepared, pixels, grids
 
     def s2_step(self, env_ids, rgbs, depths, poses, instructions, intrinsic, look_downs):
         """One System-2 consultation for the listed environments (one model call).  Returns a list with, per
         environment, an S2Output (discrete `output_action` list, or `output_pixel` + `output_latent` [1, n_query, H]) or
         the Exception that environment's host-side preparation raised."""
         results = [None] * len(env_ids)
-        prepared = []
-        for j, (e, rgb, ins, ld) in enumerate(zip(env_ids, rgbs, instructions, look_downs)):
-            try:
-                prepared.append((j, self._build_inputs(self.episodes[e], rgb, ins, ld)))
-            except Exception as exc:  # noqa: BLE001 -- reported per environment; the agent applies the retry rule
-                results[j] = exc
-        if not prepared:
-            return results
-        prompts = [inp["input_ids"][0].tolist() for _, inp in prepared]
-        pixels = torch.cat([inp["pixel_values"] for _, inp in prepared], dim=0)
-        grids = torch.cat([torch.stack(list(inp["image_grid_thw"])).reshape(-1, 3) for _, inp in prepared], dim=0)
+        if self._vl is not None:
+            prepared, pixels, grids = self._prepare_device(env_ids, rgbs, instructions, look_downs, results)
+            if not prepared:
+                return results
+            prompts = [ids for _, ids in prepared]
+        else:
+            prepared = []
+            for j, (e, rgb, ins, ld) in enumerate(zip(env_ids, rgbs, instructions, look_downs)):
+                try:
+                    prepared.append((j, self._build_inputs(self.episodes[e], rgb, ins, ld)))
+                except Exception as exc:  # noqa: BLE001 -- reported per environment; the agent applies the retry rule
+                    results[j] = exc
+            if not prepared:
+                return results
+            prompts = [inp["input_ids"][0].tolist() for _, inp in prepared]
+            pixels = torch.cat([inp["pixel_values"] for _, inp in prepared], dim=0)
+            grids = torch.cat([torch.stack(list(inp["image_grid_thw"])).reshape(-1, 3) for _, inp in prepared], dim=0)
         caches = self._caches([env_ids[j] for j, _ in prepared], [look_downs[j] for j, _ in prepared], rgbs[prepared[0][0]])
         with torch.no_grad():
             if caches is None:

@@ -1,4 +1,4 @@
-"""System-1 input preprocessing on the GPU (SURVEY.md §8 row a12).
+"""System-1 and System-2 input preprocessing on the GPU (SURVEY.md §8 rows a12 and 8f).
 
 The reference prepares every System-1 call on the host, frame by frame, with Pillow
 (internnav/agent/internvla_n1_agent.py L308-334):
@@ -10,7 +10,15 @@ for the remembered goal frame and the current frame.  `FramePreprocessor` does t
 in a handful of launches: raw uint8 / float32 frames are copied to the device once and resampled there by
 `n1_resize_rgb_u8` / `n1_resize_f32`, which reproduce Pillow's resampler bit for bit (csrc/resize.cu).  There is no
 host fallback: without the library or an H100 the constructor raises.
+
+The reference prepares every System-2 image on the host as well: the policy resizes each frame with Pillow, and the
+Qwen2-VL image processor then resizes every image of the prompt again (to `smart_resize`'s multiple of 28), rescales,
+normalises and cuts it into 14 x 14 x 2 patch rows in numpy.  `QwenImagePreprocessor` does the same on the device and
+produces the processor's rows bit for bit (converted to bf16, as the model consumes them): both resizes on
+`n1_resize_rgb_u8` (uint8 output), and rescale + normalise + patchify in one `n1_vl_patchify` launch, since after a
+uint8 resize the processor's arithmetic is a table of the 256 byte values per channel.
 """
+import math
 import ctypes
 from ctypes import c_void_p
 
@@ -42,11 +50,20 @@ def _bind(L):
     L.n1_resize_coeffs.restype = ci
     L.n1_resize_coeffs.argtypes = [ci, ci, ci, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double),
                                    ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]
+    L.n1_vl_patchify_workspace_bytes.restype = ctypes.c_size_t
+    L.n1_vl_patchify_workspace_bytes.argtypes = [ci]
+    L.n1_vl_patchify.restype = ci
+    L.n1_vl_patchify.argtypes = [ctypes.POINTER(VlImage), ci, vp, vp, ctypes.c_int64, vp, ctypes.c_size_t, vp]
     _bound = True
 
 
+class VlImage(ctypes.Structure):
+    """n1_vl_image: one resized frame of n1_vl_patchify."""
+    _fields_ = [("src_u8", c_void_p), ("h", ctypes.c_int32), ("w", ctypes.c_int32), ("row0", ctypes.c_int64)]
+
+
 RESIZE_SYMBOLS = ["n1_resize_plan_create", "n1_resize_plan_destroy", "n1_resize_workspace_bytes", "n1_resize_rgb_u8",
-                  "n1_resize_f32", "n1_resize_coeffs"]
+                  "n1_resize_f32", "n1_resize_coeffs", "n1_vl_patchify_workspace_bytes", "n1_vl_patchify"]
 
 
 def resize_coeffs(in_size, out_size):
@@ -65,13 +82,11 @@ def resize_coeffs(in_size, out_size):
             np.frombuffer(f, dtype=np.int32)[: out_size * k].reshape(out_size, k).copy())
 
 
-class FramePreprocessor:
-    def __init__(self, device="cuda:0", out_size=224):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("n1b200 has no CPU path: FramePreprocessor needs device='cuda:N'")
-        self.out = out_size
-        self._plans, self._ws = {}, {}
+class _ResizePlans:
+    """Resize plans on one device, one per (input, output) shape, created on first use and destroyed with the cache."""
+
+    def __init__(self, device):
+        self.device, self._plans = device, {}
         _bind(_lib.lib())
 
     def __del__(self):
@@ -82,14 +97,27 @@ class FramePreprocessor:
         except Exception:
             pass
 
-    def _plan(self, h, w):
-        p = self._plans.get((h, w))
+    def __call__(self, in_h, in_w, out_h, out_w):
+        key = (in_h, in_w, out_h, out_w)
+        p = self._plans.get(key)
         if p is None:
             p = c_void_p()
             with torch.cuda.device(self.device):
-                check(_lib.lib().n1_resize_plan_create(h, w, self.out, self.out, ctypes.byref(p), _lib.stream_ptr()))
-            self._plans[(h, w)] = p
+                check(_lib.lib().n1_resize_plan_create(in_h, in_w, out_h, out_w, ctypes.byref(p), _lib.stream_ptr()))
+            self._plans[key] = p
         return p
+
+
+class FramePreprocessor:
+    def __init__(self, device="cuda:0", out_size=224):
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("n1b200 has no CPU path: FramePreprocessor needs device='cuda:N'")
+        self.out = out_size
+        self._plans, self._ws = _ResizePlans(self.device), {}
+
+    def _plan(self, h, w):
+        return self._plans(h, w, self.out, self.out)
 
     def _scratch(self, key, nbytes):
         k = (key, torch.cuda.current_stream().cuda_stream)
@@ -137,3 +165,146 @@ class FramePreprocessor:
         r = self.rgb(torch.from_numpy(rgb)).view(B, 2, self.out, self.out, 3)
         d = self.depth(torch.from_numpy(dep)).view(B, 2, self.out, self.out, 1)
         return r, d
+
+
+def smart_resize(height, width, factor=28, min_pixels=56 * 56, max_pixels=28 * 28 * 1280):
+    """The size the Qwen2-VL image processor resizes an image to (transformers `smart_resize`): both sides rounded to a
+    multiple of `factor`; if that holds more than `max_pixels` pixels, both sides are scaled down by the same factor
+    and floored to a multiple (at least `factor`), if fewer than `min_pixels`, scaled up and ceiled.  An aspect ratio
+    above 200 is an error."""
+    if max(height, width) / min(height, width) > 200:
+        raise ValueError("absolute aspect ratio must be smaller than 200, got %r" % (max(height, width) / min(height, width)))
+    h_bar, w_bar = round(height / factor) * factor, round(width / factor) * factor
+    if h_bar * w_bar > max_pixels:
+        beta = math.sqrt((height * width) / max_pixels)
+        h_bar = max(factor, math.floor(height / beta / factor) * factor)
+        w_bar = max(factor, math.floor(width / beta / factor) * factor)
+    elif h_bar * w_bar < min_pixels:
+        beta = math.sqrt(min_pixels / (height * width))
+        h_bar, w_bar = math.ceil(height * beta / factor) * factor, math.ceil(width * beta / factor) * factor
+    return h_bar, w_bar
+
+
+def _is_pil_qwen2vl(image_processor):
+    """True for the PIL/numpy-backed Qwen2-VL image processor: Qwen2VLImageProcessorPil in transformers 5, the slow
+    Qwen2VLImageProcessor (not a BaseImageProcessorFast) in transformers 4.  The torchvision-backed processor resizes
+    with a different bicubic and is not reproduced."""
+    try:
+        from transformers.models.qwen2_vl import image_processing_qwen2_vl as qv
+    except ImportError:
+        return False
+    try:
+        from transformers.models.qwen2_vl.image_processing_pil_qwen2_vl import Qwen2VLImageProcessorPil
+    except ImportError:   # transformers 4
+        from transformers.image_processing_utils_fast import BaseImageProcessorFast
+        return type(image_processor) is qv.Qwen2VLImageProcessor and not isinstance(image_processor, BaseImageProcessorFast)
+    return type(image_processor) is Qwen2VLImageProcessorPil
+
+
+class QwenImagePreprocessor:
+    """The Qwen2-VL image processor of the System-2 prompt images on the GPU, bit-equal to its `pixel_values` converted
+    to bf16.  Build it with `from_hf`, which declines any processor whose arithmetic it does not reproduce."""
+
+    PATCH, TEMPORAL, MERGE = 14, 2, 2
+    ROW = 3 * TEMPORAL * PATCH * PATCH   # 1176
+
+    def __init__(self, device, lut, min_pixels, max_pixels):
+        """lut: bf16 [3, 256] = the processor's rescale + normalise of each byte value per channel."""
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("n1b200 has no CPU path: QwenImagePreprocessor needs device='cuda:N'")
+        self.min_pixels, self.max_pixels = int(min_pixels), int(max_pixels)
+        self.table = lut.to(self.device, torch.bfloat16).contiguous().reshape(3 * 256)
+        self._plans = _ResizePlans(self.device)
+
+    @classmethod
+    def supports(cls, image_processor):
+        """True for the PIL-backed Qwen2-VL image processor with Pillow bicubic resizing, resize + rescale by 1/255 +
+        normalise on, and patch 14 / temporal patch 2 / merge 2: the processor whose rows this class reproduces."""
+        from PIL import Image
+        ip = image_processor
+        if not _is_pil_qwen2vl(ip):
+            return False
+        try:
+            bicubic = int(ip.resample) == int(Image.Resampling.BICUBIC)
+        except (TypeError, ValueError):
+            return False
+        return bool(bicubic and ip.do_resize and ip.do_rescale and ip.do_normalize and ip.rescale_factor == 1 / 255) \
+            and (ip.patch_size, ip.temporal_patch_size, ip.merge_size) == (cls.PATCH, cls.TEMPORAL, cls.MERGE)
+
+    @staticmethod
+    def pixel_limits(image_processor):
+        """(min_pixels, max_pixels) of a Qwen2-VL image processor."""
+        size = getattr(image_processor, "size", None) or {}
+        return (size["shortest_edge"] if "shortest_edge" in size else image_processor.min_pixels,
+                size["longest_edge"] if "longest_edge" in size else image_processor.max_pixels)
+
+    @staticmethod
+    def lut(image_processor):
+        """float32 [3, 256]: the processor's own rescale + normalise of every byte value of each channel."""
+        ip = image_processor
+        v = np.broadcast_to(np.arange(256, dtype=np.uint8), (3, 1, 256)).copy()   # channels first
+        out = ip.normalize(ip.rescale(v, ip.rescale_factor, input_data_format="channels_first"), ip.image_mean,
+                           ip.image_std, input_data_format="channels_first")
+        return np.ascontiguousarray(out, dtype=np.float32).reshape(3, 256)
+
+    @classmethod
+    def from_hf(cls, image_processor, device):
+        """An instance for an image processor `supports` accepts on a CUDA device; None for any other processor or
+        device.  The table is converted to bf16 as the model converts the processor's float32 rows."""
+        if torch.device(device).type != "cuda" or not cls.supports(image_processor):
+            return None
+        return cls(device, torch.from_numpy(cls.lut(image_processor)).to(torch.bfloat16),
+                   *cls.pixel_limits(image_processor))
+
+    def size(self, h, w):
+        """(h, w) an image of h x w pixels is resized to."""
+        return smart_resize(h, w, self.PATCH * self.MERGE, self.min_pixels, self.max_pixels)
+
+    def grid(self, h, w):
+        """image_grid_thw row of an h x w image: (1, gh, gw) patches."""
+        oh, ow = self.size(h, w)
+        return 1, oh // self.PATCH, ow // self.PATCH
+
+    def resize(self, frames, size):
+        """frames uint8 [n, H, W, 3] (tensor or array, host or device) -> device uint8 [n, h, w, 3], Pillow's bicubic
+        `Image.resize((w, h))` of each frame."""
+        x = torch.as_tensor(frames)
+        assert x.dtype == torch.uint8 and x.ndim == 4 and x.shape[-1] == 3, "frames must be uint8 [n, H, W, 3]"
+        x = x.to(self.device).contiguous()
+        (n, h, w), (oh, ow) = x.shape[:3], size
+        L, plan = _lib.lib(), self._plans(h, w, oh, ow)
+        out = torch.empty(n, oh, ow, 3, dtype=torch.uint8, device=self.device)
+        nb = L.n1_resize_workspace_bytes(plan, n, 0)
+        ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            check(L.n1_resize_rgb_u8(plan, _lib.ptr(x), n, None, _lib.ptr(out), _lib.ptr(ws), nb, _lib.stream_ptr()))
+        return out
+
+    def __call__(self, images):
+        """images: device uint8 [H, W, 3] frames -> (pixel_values bf16 [N, 1176] on the device, image_grid_thw int64
+        [n, 3]), as `processor(images=...)` returns them.  One resize per distinct frame shape, one patchify launch."""
+        assert len(images) > 0, "no images"
+        by_shape = {}
+        for i, im in enumerate(images):
+            assert im.dtype == torch.uint8 and im.ndim == 3 and im.shape[-1] == 3, "images must be uint8 [H, W, 3]"
+            by_shape.setdefault(tuple(im.shape[:2]), []).append(i)
+        resized = [None] * len(images)
+        for (h, w), idx in by_shape.items():
+            out = self.resize(torch.stack([images[i] for i in idx]), self.size(h, w))
+            for k, i in enumerate(idx):
+                resized[i] = out[k]
+        table = (VlImage * len(images))()
+        rows = 0
+        for t, r in zip(table, resized):
+            t.src_u8, t.h, t.w, t.row0 = r.data_ptr(), r.shape[0], r.shape[1], rows
+            rows += (r.shape[0] // self.PATCH) * (r.shape[1] // self.PATCH)
+        L = _lib.lib()
+        px = torch.empty(rows, self.ROW, dtype=torch.bfloat16, device=self.device)
+        nb = L.n1_vl_patchify_workspace_bytes(len(images))
+        ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            check(L.n1_vl_patchify(table, len(images), _lib.ptr(self.table), _lib.ptr(px), rows, _lib.ptr(ws), nb,
+                                   _lib.stream_ptr()))
+        grids = torch.tensor([[1, r.shape[0] // self.PATCH, r.shape[1] // self.PATCH] for r in resized], dtype=torch.int64)
+        return px, grids
