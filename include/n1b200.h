@@ -224,6 +224,24 @@ int n1_llm_generate_pool(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, 
 int n1_image_digest(const void* pixels_bf16, int64_t cols, const int64_t* row_off_dev, int n_img, uint64_t* digest_dev,
                     void* stream);
 
+/* ---- vision features kept across calls in a caller-owned feature pool: bf16 [pool_rows, 3584] (DEVICE)
+ * Row tables are HOST int32 arrays; every entry must be a row of the pool, and each call checks that before it runs.
+ * n1_qwen_vit_rows is n1_qwen_vit writing merged row r (original token order) to feat_pool[dst_rows_host[r]] instead of
+ * out[r]; n_rows must equal n_patches / 4 and no row may appear twice.  No other pool row is written.
+ * n1_llm_generate_rows / n1_llm_generate_pool_rows are n1_llm_generate / n1_llm_generate_pool with image token i of the
+ * plan (n1_llm_plan_image_tokens of them, in plan order) read from feat_pool[image_rows_host[i]]; a row may serve several
+ * tokens of one call.  The outputs equal those of the plain entry points on the gathered features. */
+int n1_qwen_vit_rows(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels_bf16, void* feat_pool_bf16,
+                     int64_t pool_rows, const int32_t* dst_rows_host, int64_t n_rows, void* stream);
+int n1_llm_generate_rows(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feat_pool_bf16,
+                         int64_t pool_rows, const int32_t* image_rows_host, int64_t n_rows, const int32_t* eos_ids_host,
+                         int n_eos, int32_t pad_id, int32_t* tokens_host, int32_t* lens_host, void* latents_bf16,
+                         int32_t* passes_host, void* stream);
+int n1_llm_generate_pool_rows(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes,
+                              const void* feat_pool_bf16, int64_t pool_rows, const int32_t* image_rows_host, int64_t n_rows,
+                              const int32_t* eos_ids_host, int n_eos, int32_t pad_id, int32_t* tokens_host,
+                              int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
+
 /* HOST-only integer helpers (no GPU needed): the same planners, exposed for bit-exact parity tests. */
 int n1_rope_index(const int32_t* input_ids_host, int len, const int32_t* grid_thw_host, int n_img, int merge,
                   int32_t* pos3_host /* [3, len] */, int32_t* delta_host);

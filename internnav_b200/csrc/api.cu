@@ -2,6 +2,7 @@
 #include <string.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/n1b200.h"
 #include "n1_ops.h"
@@ -84,6 +85,25 @@ WeightSource to_source(const n1_tensor_desc* t, int n) {
 inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 inline const bf16* B16(const void* p) { return static_cast<const bf16*>(p); }
 inline bf16* B16(void* p) { return static_cast<bf16*>(p); }
+
+// A host row table into a feature pool of pool_rows rows: `expect` entries, each a row of the pool, and with `distinct`
+// no row twice (the rows a vision call writes).
+void check_rows(const char* fn, const void* pool, int64_t pool_rows, const int32_t* rows, int64_t n_rows, int64_t expect,
+                bool distinct) {
+  const std::string f(fn);
+  if (!pool || pool_rows <= 0 || pool_rows > INT32_MAX) throw Error(N1_ERR_ARG, f + ": null feature pool or bad pool_rows");
+  if (n_rows != expect)
+    throw Error(N1_ERR_ARG, f + ": the row table has " + std::to_string(n_rows) + " entries, the plan needs " +
+                                std::to_string(expect));
+  if (n_rows > 0 && !rows) throw Error(N1_ERR_ARG, f + ": null row table");
+  std::vector<char> seen(distinct ? (size_t)pool_rows : 0, 0);
+  for (int64_t i = 0; i < n_rows; ++i) {
+    if (rows[i] < 0 || rows[i] >= pool_rows)
+      throw Error(N1_ERR_ARG, f + ": row " + std::to_string(rows[i]) + " (entry " + std::to_string(i) +
+                                  ") is outside the pool of " + std::to_string(pool_rows) + " rows");
+    if (distinct && seen[rows[i]]++) throw Error(N1_ERR_ARG, f + ": row " + std::to_string(rows[i]) + " is written twice");
+  }
+}
 
 }  // namespace
 
@@ -425,6 +445,48 @@ int n1_image_digest(const void* pixels, int64_t cols, const int64_t* row_off, in
     if ((n_img > 0 && (!pixels || !row_off || !digest)) || n_img < 0 || cols <= 0)
       throw Error(N1_ERR_ARG, "n1_image_digest: bad arguments");
     image_digest(B16(pixels), cols, row_off, n_img, digest, S(stream));
+  });
+}
+
+int n1_qwen_vit_rows(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels, void* feat_pool,
+                     int64_t pool_rows, const int32_t* dst_rows, int64_t n_rows, void* stream) {
+  return guard([&] {
+    if (!h || !p || !pixels) throw Error(N1_ERR_ARG, "n1_qwen_vit_rows: null handle / plan / pixels");
+    const VitPlan& vp = *p->p;
+    const int unit = h->s2.dims.v_merge * h->s2.dims.v_merge;
+    check_rows("n1_qwen_vit_rows", feat_pool, pool_rows, dst_rows, n_rows, vp.host.n_patches / unit, true);
+    use(h);
+    h->s2.vit_forward(vp, ws, ws_bytes, B16(pixels), B16(feat_pool), S(stream), dst_rows);
+  });
+}
+int n1_llm_generate_rows(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feat_pool, int64_t pool_rows,
+                         const int32_t* image_rows, int64_t n_rows, const int32_t* eos, int n_eos, int32_t pad_id,
+                         int32_t* tokens, int32_t* lens, void* latents, int32_t* passes, void* stream) {
+  return guard([&] {
+    if (!h || !p) throw Error(N1_ERR_ARG, "n1_llm_generate_rows: null handle / plan");
+    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_rows: 0..4 eos ids");
+    check_rows("n1_llm_generate_rows", feat_pool, pool_rows, image_rows, n_rows, p->p->n_image_tokens, false);
+    use(h);
+    GenResult r;
+    r.tokens = tokens, r.lens = lens;
+    h->s2.llm_generate(*p->p, ws, ws_bytes, B16(feat_pool), eos, n_eos, pad_id, r, B16(latents), S(stream), image_rows);
+    if (passes) *passes = r.steps;
+  });
+}
+int n1_llm_generate_pool_rows(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes, const void* feat_pool,
+                              int64_t pool_rows, const int32_t* image_rows, int64_t n_rows, const int32_t* eos, int n_eos,
+                              int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents, int32_t* passes,
+                              void* stream) {
+  return guard([&] {
+    if (!h || !p || !pool) throw Error(N1_ERR_ARG, "n1_llm_generate_pool_rows: null handle / plan / pool");
+    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_pool_rows: 0..4 eos ids");
+    check_rows("n1_llm_generate_pool_rows", feat_pool, pool_rows, image_rows, n_rows, p->p->n_image_tokens, false);
+    use(h);
+    GenResult r;
+    r.tokens = tokens, r.lens = lens;
+    h->s2.llm_generate_pool(*p->p, *pool->p, ws, ws_bytes, B16(feat_pool), eos, n_eos, pad_id, r, B16(latents),
+                            S(stream), image_rows);
+    if (passes) *passes = r.steps;
   });
 }
 

@@ -9,13 +9,14 @@ namespace n1 {
 namespace {
 
 __global__ void gather_rows_kernel(const bf16* __restrict__ src, const int* __restrict__ idx, bf16* __restrict__ dst,
-                                   long rows, int group, int vec_per_row) {
+                                   const int* __restrict__ dst_idx, long rows, int group, int vec_per_row) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * vec_per_row) return;
   const long r = i / vec_per_row;
   const int c = i % vec_per_row;
   const long sr = (long)idx[r / group] * group + r % group;
-  reinterpret_cast<uint4*>(dst)[i] = __ldg(reinterpret_cast<const uint4*>(src) + sr * vec_per_row + c);
+  const long dr = dst_idx ? (long)dst_idx[r / group] * group + r % group : r;
+  reinterpret_cast<uint4*>(dst)[dr * vec_per_row + c] = __ldg(reinterpret_cast<const uint4*>(src) + sr * vec_per_row + c);
 }
 
 __global__ void vit_rope_table_kernel(const int* __restrict__ pos_hw, float2* __restrict__ cs, long tokens, int half,
@@ -74,14 +75,16 @@ __global__ void apply_rope_kernel(bf16* __restrict__ x, int ld, const float2* __
 
 __global__ void build_embeds_kernel(const int* __restrict__ kind, const int* __restrict__ src,
                                     const bf16* __restrict__ emb, const bf16* __restrict__ img,
-                                    const bf16* __restrict__ lat, bf16* __restrict__ out, long tokens, int vec_per_row) {
+                                    const bf16* __restrict__ lat, const int* __restrict__ img_rows,
+                                    bf16* __restrict__ out, long tokens, int vec_per_row) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= tokens * vec_per_row) return;
   const long t = i / vec_per_row;
   const int c = i % vec_per_row;
   const int k = kind[t];
   const bf16* base = k == 0 ? emb : (k == 1 ? img : lat);
-  reinterpret_cast<uint4*>(out)[i] = __ldg(reinterpret_cast<const uint4*>(base) + (long)src[t] * vec_per_row + c);
+  const long row = k == 1 && img_rows ? img_rows[src[t]] : src[t];
+  reinterpret_cast<uint4*>(out)[i] = __ldg(reinterpret_cast<const uint4*>(base) + row * vec_per_row + c);
 }
 
 
@@ -190,9 +193,10 @@ inline int nblk(long n) { return (int)((n + 255) / 256); }
 
 }  // namespace
 
-void gather_rows(const bf16* src, const int* idx, bf16* dst, long rows, int group, int cols, cudaStream_t s) {
+void gather_rows(const bf16* src, const int* idx, bf16* dst, long rows, int group, int cols, cudaStream_t s,
+                 const int* dst_idx) {
   N1_CHECK(cols % 8 == 0, "gather_rows: cols % 8");
-  gather_rows_kernel<<<nblk(rows * (cols / 8)), 256, 0, s>>>(src, idx, dst, rows, group, cols / 8);
+  gather_rows_kernel<<<nblk(rows * (cols / 8)), 256, 0, s>>>(src, idx, dst, dst_idx, rows, group, cols / 8);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }
@@ -214,10 +218,10 @@ void apply_rope(bf16* x, int ld, const float2* cs, long tokens, int heads, int h
   N1_CUDA(cudaGetLastError());
 }
 void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, const bf16* image_feats,
-                  const bf16* latent_queries, bf16* out, long tokens, int H, cudaStream_t s) {
+                  const bf16* latent_queries, bf16* out, long tokens, int H, cudaStream_t s, const int* image_rows) {
   N1_CHECK(H % 8 == 0, "build_embeds: H % 8");
-  build_embeds_kernel<<<nblk(tokens * (H / 8)), 256, 0, s>>>(kind, src, embed_tokens, image_feats, latent_queries, out,
-                                                            tokens, H / 8);
+  build_embeds_kernel<<<nblk(tokens * (H / 8)), 256, 0, s>>>(kind, src, embed_tokens, image_feats, latent_queries,
+                                                            image_rows, out, tokens, H / 8);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }

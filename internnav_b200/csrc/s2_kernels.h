@@ -4,8 +4,10 @@
 
 namespace n1 {
 
-// dst[r, :] = src[idx[r / group] * group + r % group, :]   (rows of `cols` bf16; cols % 8 == 0)
-void gather_rows(const bf16* src, const int* idx, bf16* dst, long rows, int group, int cols, cudaStream_t s);
+// dst[r, :] = src[idx[r / group] * group + r % group, :]   (rows of `cols` bf16; cols % 8 == 0).  With dst_idx the
+// destination row is dst_idx[r / group] * group + r % group instead (rows of a caller's feature pool).
+void gather_rows(const bf16* src, const int* idx, bf16* dst, long rows, int group, int cols, cudaStream_t s,
+                 const int* dst_idx = nullptr);
 // ViT 2-D rotary tables: cs[tok, j] = (cos, sin)(pos[tok, j < half/2 ? 0 : 1] * theta^(-2 (j % (half/2)) / half)),
 // j in [0, half), half = head_dim / 2.
 void vit_rope_table(const int* pos_hw, float2* cs, long tokens, int half, float theta, cudaStream_t s);
@@ -16,8 +18,10 @@ void mrope_table(const int* pos3, float2* cs, long tokens, int half, int sec_t, 
 // out[j] = x[j] c_j - x[j + hd/2] s_j ; out[j + hd/2] = x[j + hd/2] c_j + x[j] s_j, tables shared by all heads.
 void apply_rope(bf16* x, int ld, const float2* cs, long tokens, int heads, int hd, cudaStream_t s);
 // LLM input embeddings: kind[tok] 0 -> embed_tokens[src[tok]], 1 -> image_feats[src[tok]], 2 -> latent_queries[src[tok]]
+// With image_rows, image tokens read image_feats[image_rows[src[tok]]] (rows of a caller's feature pool).
 void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, const bf16* image_feats,
-                  const bf16* latent_queries, bf16* out, long tokens, int H, cudaStream_t s);
+                  const bf16* latent_queries, bf16* out, long tokens, int H, cudaStream_t s,
+                  const int* image_rows = nullptr);
 
 // ---- greedy decode with a KV cache (model.generate of internvla_n1_policy.py L169-176, then generate_latents reusing it)
 // Chunk bookkeeping: per sequence the tokens idx = len + gen - back + j (j < per_seq) -> cache rows b * slot + idx

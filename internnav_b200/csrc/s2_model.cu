@@ -308,7 +308,8 @@ LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, 
 }
 
 // ------------------------------------------------------------------------------------------------ vision tower
-size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s) const {
+size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s,
+                         const int32_t* dst_rows_host) const {
   const int Hv = dims.v_hidden, unit = dims.v_merge * dims.v_merge;
   const long N = p.host.n_patches, Nm = N / unit;
   bf16* xin = c.take<bf16>(N * patch_k_);
@@ -318,7 +319,10 @@ size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* o
   bf16* att = c.take<bf16>(N * Hv);
   bf16* hid = c.take<bf16>(N * (long)std::max(v_inter_pad_, Hv));
   bf16* m2 = c.take<bf16>(Nm * dims.v_out);
+  int* dst_rows = c.take<int>(Nm);  // last, so the buffers above sit where they sit without a row map
   if (c.dry()) return c.used();
+  if (dst_rows_host)
+    N1_CUDA(cudaMemcpyAsync(dst_rows, dst_rows_host, Nm * sizeof(int), cudaMemcpyHostToDevice, s));
 
   gather_rows(pixels, p.window_index, xin, N, unit, patch_k_, s);  // hidden_states[window_index] on merge groups
   linear(v_patch_, xin, patch_k_, x, Hv, (int)N, GemmEpilogue(), s);
@@ -353,21 +357,22 @@ size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* o
   ge.act = ACT_GELU;
   linear(merger0_, ln, Hv * unit, hid, Hv * unit, (int)Nm, ge, s);
   linear(merger2_, hid, Hv * unit, m2, dims.v_out, (int)Nm, GemmEpilogue(), s);
-  gather_rows(m2, p.reverse_index, out, Nm, 1, dims.v_out, s);  // merged[argsort(window_index)]
+  // merged[argsort(window_index)], row r to out[dst_rows[r]] with a row map
+  gather_rows(m2, p.reverse_index, out, Nm, 1, dims.v_out, s, dst_rows_host ? dst_rows : nullptr);
   return c.used();
 }
 
 size_t S2Model::ws_vit(const VitPlan& p) const { return vit_impl(Carver(nullptr, 0), p, nullptr, nullptr, nullptr); }
-void S2Model::vit_forward(const VitPlan& p, void* ws, size_t ws_bytes, const bf16* pixels, bf16* out,
-                          cudaStream_t s) const {
+void S2Model::vit_forward(const VitPlan& p, void* ws, size_t ws_bytes, const bf16* pixels, bf16* out, cudaStream_t s,
+                          const int32_t* dst_rows_host) const {
   N1_CHECK(loaded_ && ws, "vit_forward: not loaded / null workspace");
   if (ws_bytes < ws_vit(p)) throw Error(-7, "vit_forward: workspace too small");
-  vit_impl(Carver(ws, ws_bytes), p, pixels, out, s);
+  vit_impl(Carver(ws, ws_bytes), p, pixels, out, s, dst_rows_host);
 }
 
 // ------------------------------------------------------------------------------------------------ decoder prefill
 size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf16* out, cudaStream_t s,
-                         const KvCache* kv) const {
+                         const KvCache* kv, const int32_t* image_rows_host) const {
   const int H = dims.hidden, hd = dims.head_dim;
   const long T = p.tokens;
   const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd;
@@ -377,9 +382,12 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
   bf16* qkv = c.take<bf16>(T * qkv_n);
   bf16* att = c.take<bf16>(T * H);
   bf16* hid = c.take<bf16>(T * (long)inter_pad_);
+  int* image_rows = c.take<int>(p.n_image_tokens);  // last, so the buffers above sit where they sit without a row table
   if (c.dry()) return c.used();
 
-  build_embeds(p.kind, p.src, embed_, image_feats, latentq_, x, T, H, s);
+  if (image_rows_host && p.n_image_tokens > 0)
+    N1_CUDA(cudaMemcpyAsync(image_rows, image_rows_host, p.n_image_tokens * sizeof(int), cudaMemcpyHostToDevice, s));
+  build_embeds(p.kind, p.src, embed_, image_feats, latentq_, x, T, H, s, image_rows_host ? image_rows : nullptr);
   for (int l = 0; l < dims.layers; ++l) {
     const LBlock& b = lblk_[l];
     layernorm(x, H, ln, H, b.n1, nullptr, (int)T, H, dims.rms_eps, 1, s);
@@ -500,7 +508,8 @@ void S2Model::chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, 
 }
 
 size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, const int32_t* eos, int n_eos,
-                         int32_t pad, GenResult* out, bf16* latents, cudaStream_t s) const {
+                         int32_t pad, GenResult* out, bf16* latents, cudaStream_t s,
+                         const int32_t* image_rows_host) const {
   const int H = dims.hidden, hd = dims.head_dim, B = p.B, nq = dims.n_query;
   const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd, kvd = dims.kv_heads * hd, half = hd / 2;
   const int R5 = B * (nq + 1);
@@ -523,7 +532,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   if (c.dry()) return llm_impl(c, p, nullptr, nullptr, nullptr, &kv);  // prefill scratch follows the decode state
 
   // 1. prompt prefill, K/V kept; final-norm state of the last prompt token of each sequence -> g.normed [B, H]
-  llm_impl(c, p, image_feats, g.normed, s, &kv);
+  llm_impl(c, p, image_feats, g.normed, s, &kv, image_rows_host);
   std::vector<int32_t> fill((size_t)B * p.max_new, pad);
   N1_CUDA(cudaMemcpyAsync(g.out_tokens, fill.data(), fill.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   N1_CUDA(cudaMemsetAsync(g.gen, 0, B * sizeof(int), s));
@@ -568,7 +577,8 @@ size_t S2Model::ws_generate(const LlmPlan& p) const {
   return gen_impl(Carver(nullptr, 0), p, nullptr, nullptr, 0, 0, nullptr, nullptr, nullptr);
 }
 void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, const int32_t* eos,
-                           int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const {
+                           int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
+                           const int32_t* image_rows_host) const {
   N1_CHECK(loaded_ && ws, "llm_generate: not loaded / null workspace");
   N1_CHECK(p.max_new > 0, "llm_generate: the plan was not created for generation");
   N1_CHECK(!p.pool, "llm_generate: a continuation plan needs its K/V pool (n1_llm_generate_pool)");
@@ -576,13 +586,13 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
   N1_CHECK(out.tokens && out.lens, "llm_generate: null output buffers");
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate: workspace too small");
   p.wait_ready(s);
-  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s);
+  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s, image_rows_host);
   p.mark_used(s);
 }
 
 void S2Model::llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
                                 const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents,
-                                cudaStream_t s) const {
+                                cudaStream_t s, const int32_t* image_rows_host) const {
   N1_CHECK(loaded_ && ws, "llm_generate_pool: not loaded / null workspace");
   N1_CHECK(p.pool == &pool, "llm_generate_pool: the plan was not created for this K/V pool");
   if (!has_lm_head()) throw Error(-6, "llm_generate_pool: lm_head.weight was not part of the loaded state_dict");
@@ -594,7 +604,7 @@ void S2Model::llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate_pool: workspace too small");
   for (int b = 0; b < p.B; ++b) pool.valid[p.h_slot[b]] = p.h_ctx[b];  // rows past ctx are rewritten from here on
   p.wait_ready(s);
-  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s);
+  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s, image_rows_host);
   p.mark_used(s);
   // K/V exist for the prompt and every generated token but the last; the latent pass writes the last one too (and the
   // TRAJ rows after it, which are not part of the conversation)

@@ -100,8 +100,10 @@ class S2Model {
   KvPool* make_pool(int slots, int cap) const;
 
   size_t ws_vit(const VitPlan& p) const;
-  // pixels bf16 [n_patches, 3 * tpatch * patch^2] -> out bf16 [n_patches / merge^2, v_out] (original token order)
-  void vit_forward(const VitPlan& p, void* ws, size_t ws_bytes, const bf16* pixels, bf16* out, cudaStream_t s) const;
+  // pixels bf16 [n_patches, 3 * tpatch * patch^2] -> out bf16 [n_patches / merge^2, v_out] (original token order).
+  // dst_rows_host (host, n_patches / merge^2 entries, checked by the caller): merged row r goes to out[dst_rows_host[r]].
+  void vit_forward(const VitPlan& p, void* ws, size_t ws_bytes, const bf16* pixels, bf16* out, cudaStream_t s,
+                   const int32_t* dst_rows_host = nullptr) const;
   size_t ws_llm(const LlmPlan& p) const;
   // image_feats bf16 [n_image_tokens, hidden] -> out bf16 [B, n_query, hidden] (final-norm states of the TRAJ rows)
   void llm_prefill(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, bf16* out,
@@ -110,12 +112,16 @@ class S2Model {
   // K/V kept per layer, then one token per pass until every sequence emitted an eos id or max_new tokens.  When
   // `latents` is non-null the cache is reused for generate_latents(output_ids, ...) (internvla_n1.py L320-347): one more
   // pass over [last token, TRAJ x n_query] per sequence -> latents bf16 [B, n_query, hidden].  Synchronises `s`.
+  // image_rows_host (host, n_image_tokens entries, checked by the caller): image token i reads image_feats row
+  // image_rows_host[i] instead of row i (image_feats is then a feature pool).
   size_t ws_generate(const LlmPlan& p) const;
   void llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, const int32_t* eos, int n_eos,
-                    int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const;
+                    int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
+                    const int32_t* image_rows_host = nullptr) const;
   // the same on a continuation plan: K/V are read from and written to `pool` (the plan's), and pool.valid is updated
   void llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
-                         const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s) const;
+                         const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
+                         const int32_t* image_rows_host = nullptr) const;
   bool has_lm_head() const { return lm_head_.w != nullptr; }
 
   // ---- training branch, System-2 half (s2_train.cu)
@@ -146,11 +152,12 @@ class S2Model {
     float *n1 = nullptr, *n2 = nullptr;
     Lin qkv, o, gateup, down;
   };
-  size_t vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s) const;
+  size_t vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s,
+                  const int32_t* dst_rows_host = nullptr) const;
   size_t llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf16* out, cudaStream_t s,
-                  const KvCache* kv = nullptr) const;
+                  const KvCache* kv = nullptr, const int32_t* image_rows_host = nullptr) const;
   size_t gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, const int32_t* eos, int n_eos, int32_t pad,
-                  GenResult* out, bf16* latents, cudaStream_t s) const;
+                  GenResult* out, bf16* latents, cudaStream_t s, const int32_t* image_rows_host = nullptr) const;
   void chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, int per_seq, cudaStream_t s) const;
 
   Arena arena_;

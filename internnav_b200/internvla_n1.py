@@ -172,7 +172,8 @@ class InternVLAN1ForCausalLM:
         return (err * mask).sum() / mask.sum() / (err.shape[1] * err.shape[2])
 
     def generate(self, input_ids=None, pixel_values=None, image_grid_thw=None, max_new_tokens=128, do_sample=False,
-                 eos_token_id=None, pad_token_id=None, return_dict_in_generate=False, with_latents=False, **hf_kwargs):
+                 eos_token_id=None, pad_token_id=None, return_dict_in_generate=False, with_latents=False, feature_pool=None,
+                 **hf_kwargs):
         """`model.generate(**inputs, max_new_tokens=128, do_sample=False, use_cache=True, past_key_values=None,
         return_dict_in_generate=True).sequences` (internvla_n1_policy.py L169-176) for B prompts.  `sequences` is
         [B, S_max + longest generation] int64: prompt, generated ids (the eos id included), then `pad_token_id`; ragged
@@ -182,7 +183,9 @@ class InternVLAN1ForCausalLM:
         longest reusable prefix of each prompt is then neither re-encoded nor re-prefilled (qwen.System2._generate_cached),
         and the output also carries `past_key_values` (one new KVCache per prompt), `prefill_rows` and `vit_patches`.
         A None entry next to KVCaches starts a fresh conversation on an unused slot of their pool; a list of None only
-        (no pool to write to) is an uncached call."""
+        (no pool to write to) is an uncached call.  `feature_pool` (from `make_feature_pool`): the vision tower runs only
+        on the images the pool does not hold yet, and the output also carries `image_hits` (images served from the pool)
+        and `vit_patches`; outputs are byte-identical to a call without it."""
         if do_sample or hf_kwargs.get("num_beams", 1) != 1:
             raise NotImplementedError("n1b200 implements greedy search only (the reference calls do_sample=False)")
         eos = EOS_TOKEN_IDS if eos_token_id is None else \
@@ -194,6 +197,8 @@ class InternVLAN1ForCausalLM:
         if caches is not None and all(c is None for c in caches):
             caches = None
         extra = {} if caches is None else {"past_key_values": caches}
+        if feature_pool is not None:
+            extra["feature_pool"] = feature_pool
         with torch.no_grad():
             toks, lat, passes = self._s2.generate(prompts, pixel_values, grid, max_new_tokens=int(max_new_tokens),
                                                   eos_token_ids=eos, pad_token_id=pad, with_latents=with_latents, **extra)
@@ -207,6 +212,8 @@ class InternVLAN1ForCausalLM:
         if caches is not None:  # one KVCache per prompt (None: the conversation did not fit its slot)
             info = self._s2.last_cache
             out.past_key_values, out.prefill_rows, out.vit_patches = info["caches"], info["prefill_rows"], info["vit_patches"]
+        if feature_pool is not None:
+            out.image_hits, out.vit_patches = self._s2.last_features["image_hits"], self._s2.last_features["vit_patches"]
         return out if (return_dict_in_generate or with_latents) else out.sequences
 
     def make_kv_pool(self, slots, capacity):
@@ -214,6 +221,12 @@ class InternVLAN1ForCausalLM:
         allocated once: 2 * layers * kv_heads * head_dim * 2 bytes per token and slot."""
         from .qwen import KVPool
         return KVPool(self._s2, slots, capacity)
+
+    def make_feature_pool(self, rows):
+        """A vision-feature pool of `rows` merged rows (v_out bf16 each, 7 168 B at the 7B shapes), allocated once; pass it
+        as `feature_pool=` to reuse the vision tower's output for images seen in earlier calls."""
+        from .qwen import ImageFeaturePool
+        return ImageFeaturePool(self._s2, rows)
 
     def generate_with_latents(self, input_ids, pixel_values, image_grid_thw, max_new_tokens=128, **kw):
         """One System-2 call of the dual-system policy (internvla_n1_policy.py L166-195): greedy answer tokens AND the

@@ -59,6 +59,11 @@ def split_and_clean(text):
     return out
 
 
+def _image_tokens(h, w):
+    """Merged rows (= image tokens) of an h x w frame, rounded up: at least what the processor's grid gives."""
+    return math.ceil(h / 28) * math.ceil(w / 28)
+
+
 class S2Output(SimpleNamespace):
     def __init__(self):
         super().__init__(output_action=None, output_pixel=None, output_latent=None)
@@ -78,7 +83,7 @@ class _Episode:
 
 class InternVLAN1Policy:
     def __init__(self, model, processor, num_envs=1, num_history=8, resize_w=384, resize_h=384, continuous_traj=True,
-                 max_new_tokens=128, device=None):
+                 max_new_tokens=128, device=None, vision_cache_frames=0):
         self.model, self.processor = model, processor
         self.num_history, self.resize_w, self.resize_h = num_history, resize_w, resize_h
         self.continuous_traj = continuous_traj
@@ -89,6 +94,12 @@ class InternVLAN1Policy:
         # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
         self._kv_pool = None
         self._kv = [None] * num_envs
+        # vision features of images seen in earlier System-2 calls, kept for `vision_cache_frames` resized frames per
+        # environment (0: no pool, every call encodes all its images)
+        if vision_cache_frames > 0 and getattr(model, "make_feature_pool", None) is None:
+            raise ValueError("vision_cache_frames > 0 needs a model with make_feature_pool")
+        self.vision_cache_frames = int(vision_cache_frames)
+        self._feature_pool = None
         # System-2 images on the device when the processor's image arithmetic can be reproduced there
         self._vl = None
         if torch.device(self.device).type == "cuda":
@@ -106,11 +117,23 @@ class InternVLAN1Policy:
         """Tokens one environment's slot must hold: a fresh turn (num_history + 1 resized frames), the look-down frame at
         full size, two answers, the TRAJ rows, and 512 tokens for the text of both turns.  A conversation that still
         does not fit runs uncached."""
-        def img(h, w):
-            return math.ceil(h / 28) * math.ceil(w / 28)
         nq = getattr(getattr(self.model, "config", None), "n_query", 4)
-        return ((self.num_history + 1) * img(self.resize_h, self.resize_w) + img(frame_h, frame_w) +
+        return ((self.num_history + 1) * _image_tokens(self.resize_h, self.resize_w) + _image_tokens(frame_h, frame_w) +
                 2 * self.max_new_tokens + nq + 512)
+
+    def _feature_rows(self, frame_h, frame_w):
+        """Rows of the vision-feature pool: vision_cache_frames resized frames per environment, plus the most one call
+        can need at once (every environment's fresh-turn images and its look-down frame)."""
+        n, frame = len(self.episodes), _image_tokens(self.resize_h, self.resize_w)
+        return n * self.vision_cache_frames * frame + n * ((self.num_history + 1) * frame + _image_tokens(frame_h, frame_w))
+
+    def _features(self, frame):
+        """feature_pool for one call, or None without a vision cache."""
+        if self.vision_cache_frames <= 0:
+            return None
+        if self._feature_pool is None:
+            self._feature_pool = self.model.make_feature_pool(self._feature_rows(*np.asarray(frame).shape[:2]))
+        return self._feature_pool
 
     def _caches(self, env_ids, look_downs, frame):
         """past_key_values for one call, or None when the model keeps no K/V caches."""
@@ -244,12 +267,12 @@ class InternVLAN1Policy:
             pixels = torch.cat([inp["pixel_values"] for _, inp in prepared], dim=0)
             grids = torch.cat([torch.stack(list(inp["image_grid_thw"])).reshape(-1, 3) for _, inp in prepared], dim=0)
         caches = self._caches([env_ids[j] for j, _ in prepared], [look_downs[j] for j, _ in prepared], rgbs[prepared[0][0]])
+        kw = {} if caches is None else {"past_key_values": caches}
+        features = self._features(rgbs[prepared[0][0]])
+        if features is not None:
+            kw["feature_pool"] = features
         with torch.no_grad():
-            if caches is None:
-                out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens)
-            else:
-                out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens,
-                                                       past_key_values=caches)
+            out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens, **kw)
         for n, (j, _) in enumerate(prepared):
             if caches is not None:
                 self._kv[env_ids[j]] = out.past_key_values[n]

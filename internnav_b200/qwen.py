@@ -6,7 +6,9 @@ equivalents of the calls InternVLAN1ForCausalLM.generate_latents makes (internvl
 """
 import ctypes
 import itertools
+from collections import OrderedDict
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -120,6 +122,15 @@ def _bind(L):
                                        ctypes.POINTER(ctypes.c_int32), vp]
     L.n1_image_digest.restype = ctypes.c_int
     L.n1_image_digest.argtypes = [vp, ctypes.c_int64, vp, ctypes.c_int, vp, vp]
+    i64 = ctypes.c_int64
+    L.n1_qwen_vit_rows.restype = ctypes.c_int
+    L.n1_qwen_vit_rows.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, i64, i32p, i64, vp]
+    L.n1_llm_generate_rows.restype = ctypes.c_int
+    L.n1_llm_generate_rows.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, i64, i32p, i64, i32p, ctypes.c_int,
+                                       ctypes.c_int32, i32p, i32p, vp, i32p, vp]
+    L.n1_llm_generate_pool_rows.restype = ctypes.c_int
+    L.n1_llm_generate_pool_rows.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp, i64, i32p, i64, i32p, ctypes.c_int,
+                                            ctypes.c_int32, i32p, i32p, vp, i32p, vp]
     L._s2_bound = True
 
 
@@ -129,7 +140,8 @@ S2_SYMBOLS = ["n1_s2_load", "n1_vit_plan_create", "n1_vit_plan_destroy", "n1_vit
               "n1_vit_window_index", "n1_gen_plan_create", "n1_generate_workspace_bytes", "n1_s2_has_lm_head",
               "n1_llm_generate", "n1_s2_train_workspace_bytes", "n1_s2_train_forward", "n1_s2_train_backward", "n1_s2_set_latent_queries",
               "n1_kv_pool_create", "n1_kv_pool_destroy", "n1_kv_pool_bytes", "n1_kv_pool_valid", "n1_kv_pool_read", "n1_plan_rows_host", "n1_gen_plan_create_cont",
-              "n1_llm_generate_pool", "n1_image_digest"]
+              "n1_llm_generate_pool", "n1_image_digest", "n1_qwen_vit_rows", "n1_llm_generate_rows",
+              "n1_llm_generate_pool_rows"]
 
 EOS_TOKEN_IDS = (151645, 151643)  # Qwen2.5-VL generation_config.json: <|im_end|>, <|endoftext|>
 PAD_TOKEN_ID = 151643
@@ -152,6 +164,11 @@ def normalise_keys(state_dict):
 
 
 IMAGE_TOKEN_ID = 151655
+
+
+def _i32(a):
+    """ctypes int32 pointer into a C-contiguous int32 numpy array (the array must outlive the call)."""
+    return a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
 
 
 def image_spans(prompt, grids, merge=2):
@@ -248,6 +265,74 @@ class KVPool:
                 _lib.lib().n1_kv_pool_destroy(self._p)
         except Exception:
             pass
+
+
+class ImageFeaturePool:
+    """Caller-owned device memory for vision-tower output kept across calls: bf16 [rows, v_out], sized once (7 168 B per
+    row at the 7B shapes; a 392 x 392 frame is 196 rows, a 640 x 480 one 391).  An entry holds the merged rows of one
+    image, keyed by (content digest, t, h, w).  Rows are taken from a free list one at a time, so an entry's rows need
+    not be adjacent and freed rows serve any image.  A call that needs rows evicts the least recently used entries it
+    does not itself use."""
+
+    def __init__(self, s2, rows):
+        if int(rows) <= 0:
+            raise ValueError("ImageFeaturePool: rows must be positive")
+        self.rows = int(rows)
+        self.feats = torch.empty(self.rows, s2.cfg["v_out"], device=s2.device, dtype=torch.bfloat16)
+        self._free = list(range(self.rows - 1, -1, -1))  # popped from the end: lowest row first
+        self._entries = OrderedDict()                    # key -> int32 rows, least recently used first
+
+    @property
+    def bytes(self):
+        return self.feats.numel() * self.feats.element_size()
+
+    @property
+    def free_rows(self):
+        return len(self._free)
+
+    def __len__(self):
+        return len(self._entries)
+
+    def __contains__(self, key):
+        return key in self._entries
+
+    def keys(self):
+        """Entry keys, least recently used first."""
+        return list(self._entries)
+
+    def rows_of(self, key):
+        return self._entries[key].tolist()
+
+    def assign(self, keys, counts):
+        """Rows for the images of one call: image i has key keys[i] and counts[i] merged rows.  Entries that exist become
+        the most recently used; every other distinct key gets rows from the free list, after evicting least recently
+        used entries outside this call as needed.  -> (rows of each image, set of keys that got new rows: the caller
+        fills those, or discards them if it cannot).  ValueError when the call's distinct images need more rows than
+        the pool has."""
+        need = OrderedDict()
+        for k, n in zip(keys, counts):
+            need[k] = int(n)
+        total = sum(need.values())
+        if total > self.rows:
+            raise ValueError("ImageFeaturePool: one call needs %d rows of image features, the pool has %d" % (total, self.rows))
+        for k in need:
+            if k in self._entries:
+                self._entries.move_to_end(k)
+        new = [k for k in need if k not in self._entries]
+        want = sum(need[k] for k in new)
+        while len(self._free) < want:  # entries this call uses are at the end, so the oldest is never one of them
+            _, rows = self._entries.popitem(last=False)
+            self._free.extend(rows[::-1].tolist())
+        for k in new:
+            self._entries[k] = np.array([self._free.pop() for _ in range(need[k])], dtype=np.int32)
+        return [self._entries[k] for k in keys], set(new)
+
+    def discard(self, keys):
+        """Drop entries (rows whose features were never written) and return their rows to the free list."""
+        for k in keys:
+            rows = self._entries.pop(k, None)
+            if rows is not None:
+                self._free.extend(rows[::-1].tolist())
 
 
 class System2:
@@ -376,6 +461,46 @@ class System2:
         check(L.n1_qwen_vit(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(out), _lib.stream_ptr()))
         return out
 
+    def visual_rows(self, pixel_values, grid_thw, feature_pool, dst_rows):
+        """visual() writing merged row r to feature_pool.feats[dst_rows[r]] (int32, no row twice) instead of a new tensor."""
+        L = _lib.lib()
+        plan = self.vit_plan(grid_thw)
+        px = pixel_values.to(self.device, torch.bfloat16).contiguous()
+        n = L.n1_vit_plan_patches(plan)
+        assert px.shape[0] == n, "pixel_values rows (%d) do not match image_grid_thw (%d patches)" % (px.shape[0], n)
+        dst = np.ascontiguousarray(dst_rows, dtype=np.int32)
+        nb = L.n1_vit_workspace_bytes(self._h(), plan)
+        ws = self._scratch("vit", nb)
+        check(L.n1_qwen_vit_rows(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(feature_pool.feats),
+                                 feature_pool.rows, _i32(dst), len(dst), _lib.stream_ptr()))
+
+    def _pool_features(self, feature_pool, px, grid_thw, digests, images):
+        """Image features of grid_thw[i] for i in `images` (in plan order) through `feature_pool`: the images it does not
+        hold go through the vision tower in one call, into freshly taken rows.  -> (int32 row table of the plan's image
+        tokens, patches encoded, images served from the pool).  Sets self.last_features."""
+        merge2 = self.cfg["v_merge"] ** 2
+        sizes = [int(t) * int(h) * int(w) for t, h, w in grid_thw]
+        start = np.concatenate([[0], np.cumsum(sizes)]).tolist()
+        keys = [(int(digests[i]),) + tuple(int(v) for v in grid_thw[i]) for i in images]
+        rows, new = feature_pool.assign(keys, [sizes[i] // merge2 for i in images])
+        miss, seen = [], set()
+        for i, k, r in zip(images, keys, rows):
+            if k in new and k not in seen:
+                seen.add(k)
+                miss.append((i, r))
+        hits = sum(1 for k in keys if k not in new)
+        if miss:
+            try:
+                sub = torch.cat([px[start[i]:start[i + 1]] for i, _ in miss]) if len(miss) < len(grid_thw) else px
+                self.visual_rows(sub, [grid_thw[i] for i, _ in miss], feature_pool, np.concatenate([r for _, r in miss]))
+            except Exception:
+                feature_pool.discard(new)
+                raise
+        patches = sum(sizes[i] for i, _ in miss)
+        self.last_features = dict(image_hits=hits, vit_patches=patches)
+        table = np.concatenate(rows) if rows else np.zeros(0, dtype=np.int32)
+        return table, patches, hits
+
     def prefill_latents(self, prompts, image_feats, grid_thw):
         """Embedding splice + decoder prefill + last-n_query slice for B prompts -> [B, n_query, hidden] bf16."""
         L = _lib.lib()
@@ -443,23 +568,34 @@ class System2:
         return hit[0]
 
     def generate(self, prompts, pixel_values, grid_thw, max_new_tokens=128, eos_token_ids=EOS_TOKEN_IDS,
-                 pad_token_id=PAD_TOKEN_ID, with_latents=False, image_feats=None, past_key_values=None):
+                 pad_token_id=PAD_TOKEN_ID, with_latents=False, image_feats=None, past_key_values=None, feature_pool=None):
         """Greedy decode for B prompts (`model.generate(do_sample=False, max_new_tokens=...)`, internvla_n1_policy.py
         L169-176).  Returns (list of B generated-token lists, each ending with its eos id unless the budget ran out,
         latents [B, n_query, hidden] or None, decode passes run).  With `with_latents` the K/V cache of the decode is
         extended by the TRAJ tokens, which equals `generate_latents(output_ids, ...)` without a second prefill.
-        `past_key_values`: one KVCache per prompt (see _generate_cached); the call then also sets `self.last_cache`."""
+        `past_key_values`: one KVCache per prompt (see _generate_cached); the call then also sets `self.last_cache`.
+        `feature_pool`: an ImageFeaturePool; images it holds skip the vision tower, the others are encoded into it, and
+        `self.last_features` = dict(image_hits, vit_patches).  The outputs are byte-identical to a call without it."""
+        if feature_pool is not None and image_feats is not None:
+            raise ValueError("generate: image_feats and feature_pool exclude each other")
         if past_key_values is not None:
             return self._generate_cached(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
-                                         with_latents, past_key_values)
+                                         with_latents, past_key_values, feature_pool)
         L = _lib.lib()
         if not L.n1_s2_has_lm_head(self._h()):
             raise RuntimeError("generate() needs lm_head.weight in the loaded state_dict; there is no fallback")
         plan = self.gen_plan(prompts, grid_thw, max_new_tokens)
         B = len(prompts)
-        feats = self.visual(pixel_values, grid_thw) if image_feats is None else image_feats
-        feats = feats.to(self.device, torch.bfloat16).contiguous()
-        assert feats.shape[0] == L.n1_llm_plan_image_tokens(plan), "image features and image tokens do not match"
+        table = None
+        if feature_pool is not None:
+            px = pixel_values.to(self.device, torch.bfloat16).contiguous()
+            table, _, _ = self._pool_features(feature_pool, px, grid_thw, self.image_digests(px, grid_thw),
+                                              range(len(grid_thw)))
+            feats = feature_pool.feats
+        else:
+            feats = self.visual(pixel_values, grid_thw) if image_feats is None else image_feats
+            feats = feats.to(self.device, torch.bfloat16).contiguous()
+            assert feats.shape[0] == L.n1_llm_plan_image_tokens(plan), "image features and image tokens do not match"
         lat = torch.empty(B, self.cfg["n_query"], self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) \
             if with_latents else None
         nb = L.n1_generate_workspace_bytes(self._h(), plan)
@@ -468,8 +604,13 @@ class System2:
         toks = (ctypes.c_int32 * (B * int(max_new_tokens)))()
         lens = (ctypes.c_int32 * B)()
         passes = ctypes.c_int32(0)
-        check(L.n1_llm_generate(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), eos, len(eos_token_ids),
-                                int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
+        if table is None:
+            check(L.n1_llm_generate(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), eos, len(eos_token_ids),
+                                    int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
+        else:
+            check(L.n1_llm_generate_rows(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), feature_pool.rows, _i32(table),
+                                         len(table), eos, len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
+                                         ctypes.byref(passes), _lib.stream_ptr()))
         out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
         return out, lat, passes.value
 
@@ -483,7 +624,7 @@ class System2:
         return out.tolist()
 
     def _generate_cached(self, prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id, with_latents,
-                         caches):
+                         caches, feature_pool=None):
         """generate() continuing cached conversations.  caches[b] is a KVCache of one KVPool (an empty one for a fresh
         prompt; all slots distinct) or None: a fresh conversation on a slot no other entry uses (one never written if
         there is one, else the lowest; a cache held elsewhere on that slot goes stale).  Prompt b reuses reuse_length(...) rows of its slot: only the images after that
@@ -509,14 +650,15 @@ class System2:
         need = [len(p) + int(max_new_tokens) + nq for p in prompts]
         if any(n > pool.capacity for n in need):
             toks, lat, passes = self.generate(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
-                                              with_latents)
-            n_p = sum(int(t) * int(h) * int(w) for t, h, w in grid_thw)
+                                              with_latents, feature_pool=feature_pool)
+            n_p = sum(int(t) * int(h) * int(w) for t, h, w in grid_thw) if feature_pool is None else \
+                self.last_features["vit_patches"]
             self.last_cache = dict(caches=[None] * B, prefill_rows=sum(len(p) for p in prompts), vit_patches=n_p,
                                    reused=[0] * B)
             return toks, lat, passes
         px = pixel_values.to(self.device, torch.bfloat16).contiguous()
         digests = self.image_digests(px, grid_thw)
-        reused, keep_rows, keep_grids, images = [], [], [], []
+        reused, keep_rows, keep_grids, keep_idx, images = [], [], [], [], []
         gi, row = 0, 0
         for b, (p, c) in enumerate(zip(prompts, caches)):
             spans = image_spans(p, grid_thw[gi:], merge)
@@ -528,18 +670,26 @@ class System2:
                 if st >= r:
                     keep_rows.append((row, row + t * h * w))
                     keep_grids.append(grid_thw[gi + k])
+                    keep_idx.append(gi + k)
                 row += t * h * w
             reused.append(r)
             images.append({st: (n, dg) for st, n, dg in imgs})
             gi += len(spans)
-        if keep_rows:
+        table = None
+        if feature_pool is not None:
+            table, vit_patches, _ = self._pool_features(feature_pool, px, grid_thw, digests, keep_idx)
+            feats = feature_pool.feats
+        elif keep_rows:
             sub = px if len(keep_rows) == len(grid_thw) else torch.cat([px[a:e] for a, e in keep_rows])
             feats = self.visual(sub, keep_grids)
         else:
             feats = torch.empty(0, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16)
+        if feature_pool is None:
+            vit_patches = sum(e - a for a, e in keep_rows)
         slots = [c.slot for c in caches]
         plan = self._cont_plan(prompts, grid_thw, max_new_tokens, pool, reused, slots)
-        assert feats.shape[0] == L.n1_llm_plan_image_tokens(plan), "image features and image tokens do not match"
+        assert table is not None or feats.shape[0] == L.n1_llm_plan_image_tokens(plan), \
+            "image features and image tokens do not match"
         lat = torch.empty(B, nq, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) if with_latents else None
         nb = L.n1_generate_workspace_bytes(self._h(), plan)
         ws = self._scratch("gen", nb)
@@ -549,16 +699,21 @@ class System2:
         passes = ctypes.c_int32(0)
         for s_ in slots:  # the call rewrites these slots: every older handle on them is stale from here on
             pool.version[s_] += 1
-        check(L.n1_llm_generate_pool(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), eos,
-                                     len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
-                                     ctypes.byref(passes), _lib.stream_ptr()))
+        if table is None:
+            check(L.n1_llm_generate_pool(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), eos,
+                                         len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
+                                         ctypes.byref(passes), _lib.stream_ptr()))
+        else:
+            check(L.n1_llm_generate_pool_rows(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), feature_pool.rows,
+                                              _i32(table), len(table), eos, len(eos_token_ids), int(pad_token_id), toks,
+                                              lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
         out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
         new = []
         for b, p in enumerate(prompts):
             valid = pool.valid(slots[b])
             new.append(KVCache(pool, slots[b], (p + out[b])[:valid], images[b]))
         self.last_cache = dict(caches=new, prefill_rows=int(L.n1_llm_plan_tokens(plan)),
-                               vit_patches=sum(e - a for a, e in keep_rows), reused=reused)
+                               vit_patches=vit_patches, reused=reused)
         return out, lat, passes.value
 
     def _cont_plan(self, prompts, grid_thw, max_new_tokens, pool, reused, slots):
