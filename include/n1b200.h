@@ -142,8 +142,13 @@ typedef struct n1_llm_plan_s* n1_llm_plan;
 
 /* replaces: InternVLAN1ForCausalLM.from_pretrained weight placement (internvla_n1_policy.py L33-38).  Tensor names
  * follow the transformers==4.51 checkpoint layout the reference loads: "visual.*", "model.layers.*",
- * "model.embed_tokens.weight", "model.norm.weight", "model.latent_queries". */
+ * "model.embed_tokens.weight", "model.norm.weight", "model.latent_queries".
+ * "model.latent_queries" is optional: a System-2-only checkpoint (no `system1` in its config; internvla_n1_arch.py
+ * L121-123) has none (n1_s2_has_latent_queries).  On such a handle every call that embeds TRAJ rows -- n1_llm_plan_create
+ * (latent plans), n1_llm_prefill, the n1_llm_generate* calls with non-NULL latents, n1_s2_set_latent_queries and the
+ * training calls -- returns N1_ERR_WEIGHT with a message; greedy generation without latents works as usual. */
 int n1_s2_load(n1_handle h, const n1_s2_dims* dims, const n1_tensor_desc* tensors, int n, void* stream);
+int n1_s2_has_latent_queries(n1_handle h);
 
 /* Integer planning (HOST inputs; synchronous; plans are immutable and reusable across calls with equal shapes).
  * replaces: rot_pos_emb / get_window_index / cu_seqlens of the vision forward, and get_rope_index + the embedding

@@ -354,6 +354,7 @@ size_t n1_generate_workspace_bytes(n1_handle h, n1_llm_plan p) {
   return r;
 }
 int n1_s2_has_lm_head(n1_handle h) { return h && h->s2.has_lm_head() ? 1 : 0; }
+int n1_s2_has_latent_queries(n1_handle h) { return h && h->s2.has_latent_queries() ? 1 : 0; }
 int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* image_feats,
                     const int32_t* eos, int n_eos, int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents,
                     int32_t* passes, void* stream) {

@@ -192,7 +192,8 @@ void S2Model::load(const WeightSource& ws, const S2Dims& d, cudaStream_t s) {
   {
     int ld;
     embed_ = m.mat(arena_, "embed_tokens.weight", 0, d.vocab, H, &ld, s);
-    latentq_ = m.mat(arena_, "latent_queries", 0, d.n_query, H, &ld, s);
+    // a System-2-only checkpoint (no System 1 in its config) has no latent queries; generate() does not need them
+    latentq_ = m.has("latent_queries") ? m.mat(arena_, "latent_queries", 0, d.n_query, H, &ld, s) : nullptr;
   }
   inter_pad_ = (d.inter + 7) & ~7;
   lblk_.resize(d.layers);
@@ -256,6 +257,9 @@ LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, 
   const bool cont = pool != nullptr;
   N1_CHECK(cont == (ctx_in != nullptr) && cont == (slot_in != nullptr), "continuation plan: ctx, slots and pool go together");
   N1_CHECK(!cont || max_new_tokens > 0, "continuation plan: only generation plans continue a cache");
+  if (max_new_tokens < 0 && !has_latent_queries())
+    throw Error(-6, "latent plan: its prompts end in TRAJ tokens, and latent_queries was not part of the loaded state_dict "
+                    "(a System-2-only model)");
   std::unique_ptr<LlmPlan> p(new LlmPlan());
   PlanArgs a;
   a.merge = dims.v_merge, a.vocab = dims.vocab, a.n_query = dims.n_query, a.max_new = max_new_tokens;
@@ -454,6 +458,7 @@ void S2Model::llm_prefill(const LlmPlan& p, void* ws, size_t ws_bytes, const bf1
                           cudaStream_t s) const {
   N1_CHECK(loaded_ && ws, "llm_prefill: not loaded / null workspace");
   N1_CHECK(p.max_new == 0, "llm_prefill: this is a generation plan (use llm_generate)");
+  if (!has_latent_queries()) throw Error(-6, "llm_prefill: latent_queries was not part of the loaded state_dict");
   if (ws_bytes < ws_llm(p)) throw Error(-7, "llm_prefill: workspace too small");
   p.wait_ready(s);
   llm_impl(Carver(ws, ws_bytes), p, image_feats, out, s);
@@ -583,6 +588,8 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
   N1_CHECK(p.max_new > 0, "llm_generate: the plan was not created for generation");
   N1_CHECK(!p.pool, "llm_generate: a continuation plan needs its K/V pool (n1_llm_generate_pool)");
   if (!has_lm_head()) throw Error(-6, "llm_generate: lm_head.weight was not part of the loaded state_dict");
+  if (latents && !has_latent_queries())
+    throw Error(-6, "llm_generate: latents requested, but latent_queries was not part of the loaded state_dict");
   N1_CHECK(out.tokens && out.lens, "llm_generate: null output buffers");
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate: workspace too small");
   p.wait_ready(s);
@@ -596,6 +603,8 @@ void S2Model::llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t
   N1_CHECK(loaded_ && ws, "llm_generate_pool: not loaded / null workspace");
   N1_CHECK(p.pool == &pool, "llm_generate_pool: the plan was not created for this K/V pool");
   if (!has_lm_head()) throw Error(-6, "llm_generate_pool: lm_head.weight was not part of the loaded state_dict");
+  if (latents && !has_latent_queries())
+    throw Error(-6, "llm_generate_pool: latents requested, but latent_queries was not part of the loaded state_dict");
   N1_CHECK(out.tokens && out.lens, "llm_generate_pool: null output buffers");
   for (int b = 0; b < p.B; ++b)
     N1_CHECK(p.h_ctx[b] <= pool.valid[p.h_slot[b]],

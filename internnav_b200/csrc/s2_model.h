@@ -123,6 +123,8 @@ class S2Model {
                          const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
                          const int32_t* image_rows_host = nullptr) const;
   bool has_lm_head() const { return lm_head_.w != nullptr; }
+  // optional ("model.latent_queries"); every call that embeds TRAJ rows needs it and refuses to run without it
+  bool has_latent_queries() const { return latentq_ != nullptr; }
 
   // ---- training branch, System-2 half (s2_train.cu)
   // The decoder is frozen and causal: the TRAJ rows are a chunk appended to the prompt's K/V cache (exactly the latent
@@ -168,7 +170,7 @@ class S2Model {
   float* merger_ln_ = nullptr;
   Lin merger0_, merger2_;
   bf16* embed_ = nullptr;    // [vocab, hidden]
-  bf16* latentq_ = nullptr;  // [n_query, hidden]
+  bf16* latentq_ = nullptr;  // [n_query, hidden]; null for a System-2-only checkpoint
   std::vector<LBlock> lblk_;
   float* final_norm_ = nullptr;
   Lin lm_head_;  // optional ("lm_head.weight"); only generate() needs it

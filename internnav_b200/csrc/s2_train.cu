@@ -102,6 +102,7 @@ size_t S2Model::train_carve(Carver& c, const LlmPlan& p, TrainBufs& t) const {
 
 void S2Model::set_latent_queries(const bf16* src, cudaStream_t s) {
   N1_CHECK(loaded_ && src, "set_latent_queries: not loaded / null source");
+  if (!has_latent_queries()) throw Error(-6, "set_latent_queries: latent_queries was not part of the loaded state_dict");
   N1_CUDA(cudaMemcpyAsync(latentq_, src, (size_t)dims.n_query * dims.hidden * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
 }
 
@@ -116,6 +117,7 @@ size_t S2Model::ws_train(const LlmPlan& p) const {
 void S2Model::train_forward(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, bf16* states,
                             cudaStream_t s) {
   N1_CHECK(loaded_ && ws && states, "train_forward: not loaded / null buffers");
+  if (!has_latent_queries()) throw Error(-6, "train_forward: latent_queries was not part of the loaded state_dict");
   N1_CHECK(p.max_new > 0 && p.slot >= p.max_len + dims.n_query, "train_forward: needs a generation plan");
   if (ws_bytes < ws_train(p)) throw Error(-7, "train_forward: workspace too small");
   p.wait_ready(s);
@@ -173,6 +175,7 @@ void S2Model::train_forward(const LlmPlan& p, void* ws, size_t ws_bytes, const b
 void S2Model::train_backward(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* grad_states, float* grad_latent,
                              cudaStream_t s) {
   N1_CHECK(loaded_ && ws && grad_states && grad_latent, "train_backward: not loaded / null buffers");
+  if (!has_latent_queries()) throw Error(-6, "train_backward: latent_queries was not part of the loaded state_dict");
   if (ws_bytes < ws_train(p)) throw Error(-7, "train_backward: workspace too small");
   p.wait_ready(s);
   ensure_transposed(s);

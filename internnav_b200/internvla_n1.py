@@ -12,8 +12,14 @@ second full prefill in `generate_latents(output_ids, ...)` (policy L187-190).
 
 `forward()` is the training forward of the navdp_async branch on a collated batch (the backward lives in train_step.py).
 
-`system1 = "nextdit_async"` (the released DualVLN head: trajectory DiT + flow matching, nextdit.py) is served through the
-same `generate_traj`; its training branch is not built (the training step is the navdp_async one, train_step.py).
+`system1 = "nextdit_async"` (the released DualVLN head: trajectory DiT + flow matching, nextdit.py) and the synchronous
+`system1 = "nextdit"` head (the same DiT conditioned on the projected latent plan alone) are served through the same
+`generate_traj`; their training branch is not built (the training step is the navdp_async one, train_step.py).
+
+`system1 = None` (no `system1` in config.json: the released System-2 checkpoint) builds System 2 alone, as the reference
+class does (internvla_n1_arch.py L121-123): no `latent_queries`, no trajectory head.  `generate()` works as for the dual
+model; every call that needs a System 1 raises.  The class is also exported as `Qwen2_5_VLForConditionalGeneration`, the
+name under which the reference evaluator loads that checkpoint in its `system2` mode (habitat_vln_evaluator.py L123-129).
 """
 from types import SimpleNamespace
 
@@ -26,6 +32,11 @@ from .qwen import EOS_TOKEN_IDS, PAD_TOKEN_ID, QWEN25VL_7B, System2
 
 TRAJ_TOKEN_INDEX = 151667
 IMAGE_TOKEN_INDEX = 151655
+# the System-1 configurations built from config.system1 (internvla_n1_arch.py L121-145); None: System 2 only
+SYSTEM1_TYPES = (None, "navdp_async", "nextdit_async", "nextdit")
+# System-1 modules hanging directly off `.model` (internvla_n1_arch.py L131-145); the RGB branch belongs to nextdit_async
+_NEXTDIT_HEADS = ("cond_projector.", "action_encoder.", "action_decoder.", "traj_dit.")
+_NEXTDIT_ASYNC_HEADS = _NEXTDIT_HEADS + ("rgb_model.", "memory_encoder.", "rgb_resampler.")
 
 
 class _Model:
@@ -33,7 +44,7 @@ class _Model:
 
     def __init__(self, navdp, s2, config, nextdit=None):
         self.navdp = navdp          # system1 = "navdp_async"
-        self.nextdit = nextdit      # system1 = "nextdit_async": traj_dit, cond_projector, rgb_model, memory_encoder, ... in one object
+        self.nextdit = nextdit      # system1 = "nextdit_async" / "nextdit": traj_dit, cond_projector, ... in one object
         self._s2 = s2
         self.config = config
         self.device = s2.device
@@ -45,22 +56,26 @@ class _Model:
 
 class InternVLAN1ForCausalLM:
     def __init__(self, cfg=None, device="cuda:0", system1="navdp_async", predict_size=32, memory_size=2):
-        if system1 not in ("navdp_async", "nextdit_async"):
-            raise NotImplementedError("n1b200 implements system1 = 'navdp_async' and 'nextdit_async' (the reference's two "
-                                      "asynchronous System-1 heads); got %r" % (system1,))
+        if system1 == "navdp":
+            raise NotImplementedError("system1 = 'navdp' (a synchronous NavDP head) is not a configuration the reference "
+                                      "builds: its model creates no navdp module for it, so generate_traj cannot run. "
+                                      "Use 'navdp_async', 'nextdit_async', 'nextdit' or no system1 (System 2 only)")
+        if system1 not in SYSTEM1_TYPES:
+            raise NotImplementedError("n1b200 implements system1 = 'navdp_async', 'nextdit_async', 'nextdit' and None "
+                                      "(System 2 only); got %r" % (system1,))
         self.cfg = dict(QWEN25VL_7B if cfg is None else cfg)
         self.device = torch.device(device)
         self.config = SimpleNamespace(system1=system1, n_query=self.cfg["n_query"], use_cache=True,
                                       hidden_size=self.cfg["hidden"], image_token_id=IMAGE_TOKEN_INDEX)
         self._s2 = System2(self.cfg, device=device)
         navdp = nextdit = None
-        if "navdp" in system1:
+        if system1 == "navdp_async":
             navdp = NavDP_Policy_DPT_CriticSum_DAT(memory_size=memory_size, predict_size=predict_size,
                                                    vlm_token_dim=self.cfg["hidden"], navdp_version=0.1, device=device,
                                                    n_query=self.cfg["n_query"])
-        else:
+        elif system1 is not None:
             from .nextdit import NextDiTSystem1
-            nextdit = NextDiTSystem1(device=device)
+            nextdit = NextDiTSystem1(device=device, asynchronous=system1 == "nextdit_async")
         self.model = _Model(navdp, self._s2, self.config, nextdit)
 
     @classmethod
@@ -68,12 +83,13 @@ class InternVLAN1ForCausalLM:
         """`InternVLAN1ForCausalLM.from_pretrained(model_path, torch_dtype=torch.bfloat16, attn_implementation=
         "flash_attention_2", device_map={"": device})` (internvla_n1_policy.py L33-38): reads config.json and the weight
         shards of a checkpoint directory and packs them into the library.  `torch_dtype` / `attn_implementation` are
-        accepted for signature compatibility (the kernels are bf16 with fp32 accumulation; attention is the library's)."""
+        accepted for signature compatibility (the kernels are bf16 with fp32 accumulation; attention is the library's).
+        The System 1 is config.json's `system1`; without that key the model is System 2 alone, as in the reference."""
         from .checkpoint import read_checkpoint
         if device is None:
             device = (device_map or {}).get("", "cuda:0") if isinstance(device_map, dict) else (device_map or "cuda:0")
         cfg, conf, sd = read_checkpoint(model_path)
-        model = cls(cfg, device=str(device), system1=conf.get("system1", "navdp_async"),
+        model = cls(cfg, device=str(device), system1=conf.get("system1"),
                     predict_size=int(conf.get("predict_step_nums", 32)))
         model.load_state_dict(sd)
         model.name_or_path = model_path
@@ -89,6 +105,16 @@ class InternVLAN1ForCausalLM:
     def get_system1_type(self):
         return self.config.system1
 
+    @property
+    def has_system1(self):
+        return self.config.system1 is not None
+
+    def _require_system1(self, call):
+        if not self.has_system1:
+            raise RuntimeError("%s needs a System 1, and this model has none: its config.json names no `system1` (a "
+                               "System-2-only checkpoint without latent_queries or a trajectory head); use generate()"
+                               % call)
+
     def eval(self):
         return self
 
@@ -98,13 +124,12 @@ class InternVLAN1ForCausalLM:
 
     def load_state_dict(self, state_dict, strict=True):
         """Full-model state_dict in the reference checkpoint layout: `visual.*`, `model.*` (incl. `model.latent_queries`
-        and `model.navdp.*`).  `lm_head.*` is ignored (generate_latents never uses it)."""
+        and `model.navdp.*`; a System-2-only checkpoint has neither).  `lm_head.weight` goes to System 2 (generate())."""
         navdp_sd = {k[len("model.navdp."):]: v for k, v in state_dict.items() if k.startswith("model.navdp.")}
         rest = {k: v for k, v in state_dict.items() if not k.startswith("model.navdp.")}
         if self.model.nextdit is not None:
             # the NextDiT modules hang directly off `.model` in the reference (internvla_n1_arch.py L131-145)
-            heads = ("cond_projector.", "rgb_model.", "memory_encoder.", "rgb_resampler.", "action_encoder.", "action_decoder.",
-                     "traj_dit.")
+            heads = _NEXTDIT_ASYNC_HEADS if self.model.nextdit.asynchronous else _NEXTDIT_HEADS
             dit_sd = {k[len("model."):]: v for k, v in rest.items() if k.startswith("model.") and k[len("model."):].startswith(heads)}
             rest = {k: v for k, v in rest.items() if not (k.startswith("model.") and k[len("model."):].startswith(heads))}
             self.model.nextdit.load_state_dict(dit_sd)
@@ -113,8 +138,11 @@ class InternVLAN1ForCausalLM:
             self.model.navdp.load_state_dict(navdp_sd)
 
     def load_parts(self, s2_state_dict, system1_state_dict):
+        if not self.has_system1 and system1_state_dict:
+            raise ValueError("load_parts: this model has no System 1 to load system1_state_dict into")
         self._s2.load_state_dict(s2_state_dict)
-        (self.model.navdp if self.model.nextdit is None else self.model.nextdit).load_state_dict(system1_state_dict)
+        if self.has_system1:
+            (self.model.navdp if self.model.nextdit is None else self.model.nextdit).load_state_dict(system1_state_dict)
 
     # ------------------------------------------------------------------ hot path
     @staticmethod
@@ -126,6 +154,7 @@ class InternVLAN1ForCausalLM:
     def generate_latents(self, input_ids, pixel_values, image_grid_thw):
         """internvla_n1.py L320-347.  input_ids: [B, S] tensor (equal lengths) or a list of B token-id lists (ragged);
         pixel_values [sum patches, 1176]; image_grid_thw [n_img, 3] in prompt order -> [B, n_query, hidden]."""
+        self._require_system1("generate_latents")
         grid = image_grid_thw.tolist() if torch.is_tensor(image_grid_thw) else image_grid_thw
         with torch.no_grad():
             return self._s2.generate_latents(self._prompts(input_ids), pixel_values, grid)
@@ -134,6 +163,7 @@ class InternVLAN1ForCausalLM:
                       num_inference_steps=10, num_sample_trajs=32, x_init=None, step_noise=None):
         """internvla_n1.py L349-441: the nextdit branch (L359-432, flow-matching Euler over the trajectory DiT with
         classifier-free guidance) or the navdp branch (L434-441) -> [num_sample_trajs * B, predict_size, 3]."""
+        self._require_system1("generate_traj")
         if self.model.nextdit is not None:
             return self.model.nextdit.generate_traj(traj_latents.to(self.device), images_dp, depths_dp,
                                                     predict_step_nums=predict_step_nums, guidance_scale=guidance_scale,
@@ -147,6 +177,7 @@ class InternVLAN1ForCausalLM:
                          step_noise=None):
         """One full policy step for B environments: System-2 latent plan -> System-1 trajectories -> action ids.
         Returns (trajectories [32B, T, 3], list of B action lists (<= 4 non-zero ids each, [] => action -1))."""
+        self._require_system1("dual_system_step")
         lat = self.generate_latents(input_ids, pixel_values, image_grid_thw)
         traj = self.generate_traj(lat, images_dp, depths_dp, x_init=x_init, step_noise=step_noise)
         acts = [s1_action_list(a) for a in batched_traj_to_actions(traj, lat.shape[0], max_actions=4)]
@@ -188,6 +219,8 @@ class InternVLAN1ForCausalLM:
         and `vit_patches`; outputs are byte-identical to a call without it."""
         if do_sample or hf_kwargs.get("num_beams", 1) != 1:
             raise NotImplementedError("n1b200 implements greedy search only (the reference calls do_sample=False)")
+        if with_latents:
+            self._require_system1("generate(with_latents=True)")
         eos = EOS_TOKEN_IDS if eos_token_id is None else \
             (tuple(eos_token_id) if isinstance(eos_token_id, (list, tuple)) else (int(eos_token_id),))
         pad = PAD_TOKEN_ID if pad_token_id is None else int(pad_token_id)
@@ -232,6 +265,7 @@ class InternVLAN1ForCausalLM:
         """One System-2 call of the dual-system policy (internvla_n1_policy.py L166-195): greedy answer tokens AND the
         latent plan `generate_latents(output_ids, pixel_values, image_grid_thw)`, sharing one vision pass, one prefill
         and the decode's K/V cache.  -> namespace(sequences, generated, latents [B, n_query, hidden], decode_passes)."""
+        self._require_system1("generate_with_latents")
         return self.generate(input_ids, pixel_values, image_grid_thw, max_new_tokens=max_new_tokens, with_latents=True,
                              return_dict_in_generate=True, **kw)
 
@@ -263,6 +297,7 @@ class InternVLAN1ForCausalLM:
         logits=None, traj_hidden_states).  This call is the forward (loss value, no autograd graph); the optimisation step --
         backward kernels, gradient exchange, AdamW -- is `train_step.DualSystemTrainer.step` (SURVEY.md §8 row a13); `logits` (computed but unused by this branch in the reference, L229) are not produced.
         `noise` / `timesteps` inject the draws of `sample_noise` (navdp.py L165-175) for parity tests."""
+        self._require_system1("forward")
         if labels is None or t_s_pos is None or traj_images is None:
             raise NotImplementedError("forward() implements the training branch (labels + t_s_pos + traj_* given); for "
                                       "inference use generate() / generate_latents() / generate_traj()")
@@ -272,6 +307,9 @@ class InternVLAN1ForCausalLM:
         return SimpleNamespace(loss=loss, logits=None, traj_hidden_states=hs)
 
     __call__ = forward
+
+
+Qwen2_5_VLForConditionalGeneration = InternVLAN1ForCausalLM
 
 
 class S1Output(SimpleNamespace):

@@ -143,10 +143,17 @@ def _enc_layer(p, D, ff):
     return out
 
 
-def nextdit_shapes(dim=384, layers=12, heads=6, latent=768, vlm_token_dim=3584, ffn=1024):
+NEXTDIT_ASYNC_ONLY = ("rgb_model.", "memory_encoder.", "rgb_resampler.")
+
+
+def nextdit_shapes(dim=384, layers=12, heads=6, latent=768, vlm_token_dim=3584, ffn=1024, asynchronous=True):
     """Tensors of the `nextdit_async` System 1 under the reference's attribute paths below `InternVLAN1ForCausalLM.model`
     (internvla_n1_arch.py L131-145: cond_projector, rgb_model, memory_encoder, rgb_resampler, action_encoder / decoder,
-    traj_dit = NextDiTCrossAttn(latent_embedding_size=768), nextdit_crossattn_traj.py L46-82)."""
+    traj_dit = NextDiTCrossAttn(latent_embedding_size=768), nextdit_crossattn_traj.py L46-82).  `asynchronous=False`:
+    the synchronous `nextdit` head, which has no rgb_model / memory_encoder / rgb_resampler (L141-145)."""
+    if not asynchronous:
+        full = nextdit_shapes(dim, layers, heads, latent, vlm_token_dim, ffn)
+        return OrderedDict((k, v) for k, v in full.items() if not k.startswith(NEXTDIT_ASYNC_ONLY))
     D, L = dim, latent
     items = [("cond_projector.0.weight", (L, vlm_token_dim)), ("cond_projector.0.bias", (L,)),
              ("cond_projector.2.weight", (L, L)), ("cond_projector.2.bias", (L,))]

@@ -1,4 +1,5 @@
-"""NextDiT System 1 (`system1 = "nextdit_async"`, the released DualVLN trajectory head) on libn1b200.so.
+"""NextDiT System 1 (`system1 = "nextdit_async"`, the released DualVLN trajectory head, and the synchronous
+`system1 = "nextdit"` head) on libn1b200.so.
 
 Mirrors the nextdit branch of `InternVLAN1ForCausalLM.generate_traj` (internnav/model/basemodel/internvla_n1/
 internvla_n1.py L349-432) for a batch of environments:
@@ -8,6 +9,11 @@ internvla_n1.py L349-432) for a batch of environments:
       -> 10 flow-matching Euler steps of the 12-block LuminaNextDiT (nextdit_traj.py L125-178, L296-368) over
          B * Ns trajectories of 32 steps, classifier-free guidance batch [null | cond]
       -> trajectories [B * Ns, 32, 3]
+
+The synchronous head (`asynchronous=False`) has no RGB branch (no rgb_model / memory_encoder / rgb_resampler,
+internvla_n1_arch.py L131-145): its condition tokens are cond_projector(latents) alone, [B, n_query, 768] (internvla_n1.py
+L361-382), and the frames are accepted and ignored, as in the reference.  The sampler is the same code with 4 keys per
+cross-attention instead of 36.
 
 Every matrix product, attention, normalisation and the sampler update run in the library (wgmma GEMM, the attention
 kernels, csrc/nextdit_kernels.cu); this module is the schedule -- it orders the launches, owns the packed weights and the
@@ -88,10 +94,13 @@ def fold_head(W2, b2, Wd, bd):
 
 
 class NextDiTSystem1:
-    """state_dict keys: internnav_b200.manifest.nextdit_shapes() (the reference's attribute paths below `.model`)."""
+    """state_dict keys: internnav_b200.manifest.nextdit_shapes(asynchronous=...) (the reference's attribute paths below
+    `.model`).  asynchronous=True: `system1 = "nextdit_async"`; False: `system1 = "nextdit"`."""
+    asynchronous = True
 
-    def __init__(self, device="cuda:0", num_inference_steps=10):
+    def __init__(self, device="cuda:0", num_inference_steps=10, asynchronous=True):
         self.device = torch.device(device)
+        self.asynchronous = bool(asynchronous)
         if self.device.type != "cuda":
             raise RuntimeError("n1b200 has no CPU path: NextDiTSystem1 needs device='cuda:N'")
         _lib.lib()
@@ -101,7 +110,7 @@ class NextDiTSystem1:
     # ------------------------------------------------------------------------------------------------ weights
     def load_state_dict(self, sd):
         from .manifest import nextdit_shapes
-        want = nextdit_shapes()
+        want = nextdit_shapes(asynchronous=self.asynchronous)
         missing = [k for k in want if k not in sd and "mask_token" not in k and "visual_proj" not in k and "patch_embedder" not in k]
         if missing:
             raise KeyError("NextDiT state_dict misses %d tensors, e.g. %s" % (len(missing), missing[:3]))
@@ -111,6 +120,15 @@ class NextDiTSystem1:
         w = {}
         for k in ("cond_projector.0", "cond_projector.2"):
             w[k + ".w"], w[k + ".b"] = b16(sd[k + ".weight"]), f32(k + ".bias")
+        if self.asynchronous:
+            self._load_rgb_branch(sd, w, f32, b16)
+        self._load_dit(sd, w, f32, b16)
+        self.w = w
+        self._pos_cache = {}
+        return self
+
+    def _load_rgb_branch(self, sd, w, f32, b16):
+        """DINOv2 ViT-S/14, MemoryEncoder and QFormer of the asynchronous head."""
         # DINOv2 ViT-S/14: im2col weight per channel with the ImageNet normalisation folded in
         Wpe, bpe = fold_patch_embed(f32("rgb_model.patch_embed.proj.weight"), f32("rgb_model.patch_embed.proj.bias"))
         w["vit.patch.w"], w["vit.patch.b"] = b16(Wpe), bpe
@@ -138,7 +156,10 @@ class NextDiTSystem1:
                 w[q + n + ".w"], w[q + n + ".b"] = b16(sd[p + n + ".weight"]), f32(p + n + ".bias")
             for n in ("norm1", "norm2", "norm3") if dec else ("norm1", "norm2"):
                 w[q + n + ".w"], w[q + n + ".b"] = f32(p + n + ".weight"), f32(p + n + ".bias")
-        # trajectory DiT
+
+    def _load_dit(self, sd, w, f32, b16):
+        """Trajectory DiT, action encoder and decoder (both heads)."""
+        dev = self.device
         p = "traj_dit.model."
         for n in ("caption_projection.linear_1", "caption_projection.linear_2", "time_caption_embed.timestep_embedder.linear_1",
                   "time_caption_embed.timestep_embedder.linear_2", "time_caption_embed.caption_embedder.1", "norm_out.linear_1"):
@@ -168,9 +189,6 @@ class NextDiTSystem1:
                            f32("action_decoder.bias"))
         w["head.w"], w["head.b"] = b16(Wh), bh
         w["enc.w"], w["enc.b"] = f32("action_encoder.weight"), f32("action_encoder.bias")
-        self.w = w
-        self._pos_cache = {}
-        return self
 
     # ------------------------------------------------------------------------------------------------ building blocks
     def _lin(self, x, name, act=ACT_NONE, residual=None, gamma=None, bias=True):
@@ -223,11 +241,14 @@ class NextDiTSystem1:
         return t.view(n, 257, DIM)[:, 1:].contiguous()
 
     def condition_tokens(self, traj_latents, images_dp):
-        """internvla_n1.py L363-382 per environment: -> bf16 [B, 36, 768]."""
+        """internvla_n1.py L363-382 per environment: -> bf16 [B, 36, 768]; the synchronous head: cond_projector(latents)
+        alone, [B, n_query, 768] (images_dp is not read)."""
         assert self.w is not None, "load_state_dict first"
         B = traj_latents.shape[0]
         lat = traj_latents.to(self.device, torch.bfloat16).reshape(B * traj_latents.shape[1], -1).contiguous()
         lat = self._lin(self._lin(lat, "cond_projector.0", act=ACT_GELU_TANH), "cond_projector.2")
+        if not self.asynchronous:
+            return lat.view(B, -1, LATENT)
         img = images_dp.to(self.device, torch.float32)
         assert tuple(img.shape[1:]) == (2, 224, 224, 3), "images_dp is [B, 2, 224, 224, 3] ([pixel-goal frame, current frame])"
         feat = self._vit(img.reshape(B * 2, 224, 224, 3)).view(B, 512, DIM)
@@ -375,7 +396,8 @@ class NextDiTSystem1:
 
     def generate_traj(self, traj_latents, images_dp, depths_dp=None, predict_step_nums=32, guidance_scale=1.0,
                       num_inference_steps=10, num_sample_trajs=32, x_init=None, exact_cfg=False, graph=None):
-        """Signature of the reference's generate_traj (depths_dp is unused by this System 1).  `x_init` injects the initial
+        """Signature of the reference's generate_traj (depths_dp is unused by this System 1, images_dp by the synchronous
+        head).  `x_init` injects the initial
         noise (tests); by default it is drawn on the device in the latents' dtype as the reference does."""
         B = traj_latents.shape[0]
         if x_init is None:

@@ -17,6 +17,10 @@ history keeps device uint8 frames, the frames of one call are uploaded and resiz
 environments come from one `QwenImagePreprocessor` call, bit-equal to the processor's.  The processor then only
 tokenises the chat text, with each image placeholder expanded as it would expand it.  Otherwise every frame is a PIL
 image and the processor prepares each environment's prompt on the host, as in the reference.
+
+A model without a System 1 (`system1 = None`, the System-2-only checkpoint) is served as the reference evaluator serves it
+in its `system2` mode: `s2_step` calls `generate` alone (no TRAJ pass), pixel answers carry no latent plan
+(`output_latent` is None), and `s1_step_latent` raises.
 """
 import copy
 import itertools
@@ -89,6 +93,7 @@ class InternVLAN1Policy:
         self.continuous_traj = continuous_traj
         self.max_new_tokens = max_new_tokens
         self.device = device if device is not None else getattr(model, "device", "cpu")
+        self.has_system1 = getattr(model, "has_system1", True)
         self.episodes = [_Episode() for _ in range(num_envs)]
         # K/V cache of each environment's last System-2 conversation, passed back on its look-down turn only (the turn
         # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
@@ -246,8 +251,8 @@ class InternVLAN1Policy:
 
     def s2_step(self, env_ids, rgbs, depths, poses, instructions, intrinsic, look_downs):
         """One System-2 consultation for the listed environments (one model call).  Returns a list with, per
-        environment, an S2Output (discrete `output_action` list, or `output_pixel` + `output_latent` [1, n_query, H]) or
-        the Exception that environment's host-side preparation raised."""
+        environment, an S2Output (discrete `output_action` list, or `output_pixel` + `output_latent` [1, n_query, H];
+        None without a System 1) or the Exception that environment's host-side preparation raised."""
         results = [None] * len(env_ids)
         if self._vl is not None:
             prepared, pixels, grids = self._prepare_device(env_ids, rgbs, instructions, look_downs, results)
@@ -272,7 +277,11 @@ class InternVLAN1Policy:
         if features is not None:
             kw["feature_pool"] = features
         with torch.no_grad():
-            out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens, **kw)
+            if self.has_system1:
+                out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens, **kw)
+            else:
+                out = self.model.generate(prompts, pixels, grids, max_new_tokens=self.max_new_tokens,
+                                          return_dict_in_generate=True, **kw)
         for n, (j, _) in enumerate(prepared):
             if caches is not None:
                 self._kv[env_ids[j]] = out.past_key_values[n]
@@ -283,7 +292,7 @@ class InternVLAN1Policy:
                 if re.search(r"\d", ep.llm_output):   # pixel goal "y x" -> [x, y] plus the latent plan (L179-190)
                     coord = [int(c) for c in re.findall(r"\d+", ep.llm_output)]
                     res.output_pixel = np.array([int(coord[1]), int(coord[0])])
-                    res.output_latent = out.latents[n:n + 1]
+                    res.output_latent = out.latents[n:n + 1] if self.has_system1 else None
                 else:
                     res.output_action = parse_actions(ep.llm_output)
                 results[j] = res
@@ -295,6 +304,9 @@ class InternVLAN1Policy:
     def s1_step_latent(self, env_ids, rgbs, depths, latents):
         """L200-215 for the listed environments in one generate_traj call: rgbs / depths are the per-environment
         [1, 2, 224, 224, 3] / [1, 2, 224, 224, 1] stacks of the agent, latents the [1, n_query, H] plans."""
+        if not self.has_system1:
+            raise RuntimeError("s1_step_latent needs a System 1, and the policy's model has none (system1 = None: a "
+                               "System-2-only checkpoint answers with discrete actions or pixel goals only)")
         lat = torch.cat([l.reshape(1, *l.shape[-2:]) for l in latents], dim=0)
         rgb = torch.cat([torch.as_tensor(r).reshape(1, *torch.as_tensor(r).shape[-4:]) for r in rgbs], dim=0)
         dep = torch.cat([torch.as_tensor(d).reshape(1, *torch.as_tensor(d).shape[-4:]) for d in depths], dim=0)

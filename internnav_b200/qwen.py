@@ -84,6 +84,8 @@ def _bind(L):
     L.n1_generate_workspace_bytes.argtypes = [vp, vp]
     L.n1_s2_has_lm_head.restype = ctypes.c_int
     L.n1_s2_has_lm_head.argtypes = [vp]
+    L.n1_s2_has_latent_queries.restype = ctypes.c_int
+    L.n1_s2_has_latent_queries.argtypes = [vp]
     L.n1_llm_generate.restype = ctypes.c_int
     L.n1_llm_generate.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
                                   ctypes.c_int32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
@@ -138,6 +140,7 @@ S2_SYMBOLS = ["n1_s2_load", "n1_vit_plan_create", "n1_vit_plan_destroy", "n1_vit
               "n1_llm_plan_destroy", "n1_llm_plan_tokens", "n1_llm_plan_image_tokens", "n1_llm_plan_positions",
               "n1_vit_workspace_bytes", "n1_llm_workspace_bytes", "n1_qwen_vit", "n1_llm_prefill", "n1_rope_index",
               "n1_vit_window_index", "n1_gen_plan_create", "n1_generate_workspace_bytes", "n1_s2_has_lm_head",
+              "n1_s2_has_latent_queries",
               "n1_llm_generate", "n1_s2_train_workspace_bytes", "n1_s2_train_forward", "n1_s2_train_backward", "n1_s2_set_latent_queries",
               "n1_kv_pool_create", "n1_kv_pool_destroy", "n1_kv_pool_bytes", "n1_kv_pool_valid", "n1_kv_pool_read", "n1_plan_rows_host", "n1_gen_plan_create_cont",
               "n1_llm_generate_pool", "n1_image_digest", "n1_qwen_vit_rows", "n1_llm_generate_rows",
@@ -383,6 +386,11 @@ class System2:
                 L.n1_destroy(self._handle)
         except Exception:
             pass
+
+    @property
+    def has_latent_queries(self):
+        """Whether the loaded state_dict held `model.latent_queries` (a System-2-only checkpoint has none)."""
+        return bool(_lib.lib().n1_s2_has_latent_queries(self._h()))
 
     def _h(self):
         if self._handle is None:

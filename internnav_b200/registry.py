@@ -38,6 +38,12 @@ class InternVLAN1Net(InternVLAN1Policy):
         super().__init__(model, processor, num_envs=int(m.get("env_num", 1)), num_history=int(m.get("num_history", 8)),
                          resize_w=int(m.get("resize_w", 384)), resize_h=int(m.get("resize_h", 384)),
                          continuous_traj=bool(m.get("continuous_traj", True)), device=device)
+        # the System 1 is the checkpoint's (config.json `system1`); a setting that names another one is an error
+        system1 = getattr(getattr(model, "config", None), "system1", m.get("system1"))
+        if m.get("system1", system1) != system1:
+            raise ValueError("model_settings system1=%r, but the checkpoint at %s has system1=%r"
+                             % (m["system1"], m["model_path"], system1))
+        m["system1"] = system1
         self.model_config = SimpleNamespace(**m)
 
 
