@@ -139,16 +139,18 @@ typedef struct {
 
 typedef struct n1_vit_plan_s* n1_vit_plan;
 typedef struct n1_llm_plan_s* n1_llm_plan;
+typedef struct n1_kv_pool_s* n1_kv_pool;
 
 /* replaces: InternVLAN1ForCausalLM.from_pretrained weight placement (internvla_n1_policy.py L33-38).  Tensor names
  * follow the transformers==4.51 checkpoint layout the reference loads: "visual.*", "model.layers.*",
- * "model.embed_tokens.weight", "model.norm.weight", "model.latent_queries".
+ * "model.embed_tokens.weight", "model.norm.weight", "model.latent_queries", and "lm_head.weight" for n1_llm_generate.
  * "model.latent_queries" is optional: a System-2-only checkpoint (no `system1` in its config; internvla_n1_arch.py
  * L121-123) has none (n1_s2_has_latent_queries).  On such a handle every call that embeds TRAJ rows -- n1_llm_plan_create
- * (latent plans), n1_llm_prefill, the n1_llm_generate* calls with non-NULL latents, n1_s2_set_latent_queries and the
- * training calls -- returns N1_ERR_WEIGHT with a message; greedy generation without latents works as usual. */
+ * of a latent plan, n1_llm_prefill, n1_llm_generate with non-NULL latents, n1_s2_set_latent_queries and the training
+ * calls -- returns N1_ERR_WEIGHT with a message; greedy generation without latents works as usual. */
 int n1_s2_load(n1_handle h, const n1_s2_dims* dims, const n1_tensor_desc* tensors, int n, void* stream);
 int n1_s2_has_latent_queries(n1_handle h);
+int n1_s2_has_lm_head(n1_handle h);
 
 /* Integer planning (HOST inputs; synchronous; plans are immutable and reusable across calls with equal shapes).
  * replaces: rot_pos_emb / get_window_index / cu_seqlens of the vision forward, and get_rope_index + the embedding
@@ -156,102 +158,83 @@ int n1_s2_has_latent_queries(n1_handle h);
 int n1_vit_plan_create(n1_handle h, const int32_t* grid_thw_host, int n_img, n1_vit_plan* out, void* stream);
 void n1_vit_plan_destroy(n1_vit_plan p);
 int64_t n1_vit_plan_patches(n1_vit_plan p);
-/* input_ids_host: prompts packed back to back (WITHOUT the TRAJ tokens, which are appended per sequence),
- * lens_host[B]; image placeholders (151655) are matched to image_grid_thw rows in order across the batch. */
+/* A decoder plan over B prompts: input_ids_host packed back to back, lens_host[B]; image placeholders (151655) are
+ * matched to image_grid_thw rows in order across the batch.
+ *   max_new_tokens == 0: a latent plan for n1_llm_prefill; n_query TRAJ tokens are appended to every prompt.
+ *   max_new_tokens >= 1: a generation plan for n1_llm_generate over the prompts alone, with K/V cache rows for
+ *     max_new_tokens + n_query more tokens per sequence.
+ *   pool, reused_host, slots_host: all NULL, or all given for a generation plan that continues conversations on a K/V
+ *     pool.  Sequence b then lives in pool slot slots_host[b] (the slots of one batch differ), whose first reused_host[b]
+ *     prompt tokens already hold its K/V (0: a fresh sequence).  Positions come from the whole prompt, but only the rows
+ *     after that prefix are embedded and prefilled, so the image features cover only the images after it.  The prefix
+ *     may not end inside an image, and prompt + max_new_tokens + n_query must fit the pool's capacity. */
 int n1_llm_plan_create(n1_handle h, const int32_t* input_ids_host, const int32_t* lens_host, int B,
-                       const int32_t* grid_thw_host, int n_img, n1_llm_plan* out, void* stream);
+                       const int32_t* grid_thw_host, int n_img, int max_new_tokens, n1_kv_pool pool,
+                       const int32_t* reused_host, const int32_t* slots_host, n1_llm_plan* out, void* stream);
 void n1_llm_plan_destroy(n1_llm_plan p);
-int64_t n1_llm_plan_tokens(n1_llm_plan p);       /* total tokens incl. appended TRAJ tokens */
-int64_t n1_llm_plan_image_tokens(n1_llm_plan p);
+int64_t n1_llm_plan_tokens(n1_llm_plan p);       /* rows the plan embeds and prefills (latent plans: incl. TRAJ tokens) */
+int64_t n1_llm_plan_image_tokens(n1_llm_plan p); /* image tokens among them: the feature rows a call reads */
 /* copies the [3, tokens] position ids (int32) and [B] mrope deltas to HOST buffers (parity with get_rope_index) */
 int n1_llm_plan_positions(n1_llm_plan p, int32_t* pos3_host, int32_t* delta_host);
 
 size_t n1_vit_workspace_bytes(n1_handle h, n1_vit_plan p);
+/* scratch of n1_llm_prefill on a latent plan, of n1_llm_generate on a generation plan */
 size_t n1_llm_workspace_bytes(n1_handle h, n1_llm_plan p);
 
 /* replaces: self.visual(pixel_values, grid_thw=image_grid_thw)     (internvla_n1.py L132, L330)
- * pixels bf16 [n_patches, 1176] -> out bf16 [n_patches / 4, 3584] */
+ * pixels bf16 [n_patches, 1176] -> n_patches / 4 merged rows of 3584 bf16 (original token order) in out [out_rows, 3584].
+ * dst_rows_host NULL: merged row r goes to out[r]; n_rows must be 0 and out_rows n_patches / 4.
+ * Otherwise out is a feature pool kept across calls and merged row r goes to out[dst_rows_host[r]]: the HOST int32 table
+ * has n_rows == n_patches / 4 entries, each a row of the pool and none twice, and no other pool row is written. */
 int n1_qwen_vit(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels_bf16, void* out_bf16,
-                void* stream);
+                int64_t out_rows, const int32_t* dst_rows_host, int64_t n_rows, void* stream);
 /* replaces: embed splice + self.model(inputs_embeds, position_ids) + hidden_states[-1][:, -n_query:]
  *                                                                   (internvla_n1.py L322-345)
- * image_feats bf16 [n_image_tokens, 3584] -> latents bf16 [B, n_query, 3584] */
+ * on a latent plan: image_feats bf16 [n_image_tokens, 3584] -> latents bf16 [B, n_query, 3584] */
 int n1_llm_prefill(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* image_feats_bf16,
                    void* latents_bf16, void* stream);
 
-/* ---- greedy decode of System 2 with KV reuse into the latent plan
- * replaces: self.model.generate(**inputs, max_new_tokens=128, do_sample=False, use_cache=True)
+/* replaces: self.model.generate(**inputs, max_new_tokens=128, do_sample=False, use_cache=True)
  *                                                          (internvla_n1_policy.py L169-176; habitat_vln_evaluator.py L418-448)
  *           followed by self.model.generate_latents(output_ids, pixel_values, image_grid_thw)   (policy L187-190),
  *           which in the reference repeats the vision tower and the whole prefill; here the K/V cache of the decode is
  *           extended by [last token, TRAJ x n_query] instead.
- * A generation plan is an n1_llm_plan created over the prompts alone (no TRAJ tokens) with cache slots for
- * max_new_tokens + n_query more rows per sequence; n1_llm_prefill refuses it and n1_llm_generate refuses latent plans.
- * The state_dict given to n1_s2_load must hold "lm_head.weight" (n1_s2_has_lm_head). */
-int n1_gen_plan_create(n1_handle h, const int32_t* input_ids_host, const int32_t* lens_host, int B,
-                       const int32_t* grid_thw_host, int n_img, int max_new_tokens, n1_llm_plan* out, void* stream);
-size_t n1_generate_workspace_bytes(n1_handle h, n1_llm_plan p);
-int n1_s2_has_lm_head(n1_handle h);
-/* image_feats bf16 [n_image_tokens, 3584] (n1_qwen_vit output).  eos_ids_host: <= 4 ids (Qwen2.5-VL generation
- * config: 151645, 151643); a sequence stops after emitting one of them (the id is part of its output) or after
- * max_new_tokens.  tokens_host [B, max_new_tokens] int32 (tail filled with pad_id), lens_host [B] = tokens emitted.
- * latents_bf16 (device, [B, n_query, 3584]) may be NULL.  *passes_host (nullable) = decode passes run.  The call
- * synchronises `stream` (the stop test reads a device counter after every token). */
-int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* image_feats_bf16,
-                    const int32_t* eos_ids_host, int n_eos, int32_t pad_id, int32_t* tokens_host, int32_t* lens_host,
-                    void* latents_bf16, int32_t* passes_host, void* stream);
+ * Greedy decode on a generation plan (a latent plan is refused); the handle needs "lm_head.weight" (n1_s2_has_lm_head).
+ * feats bf16 [feat_rows, 3584] holds the image features (n1_qwen_vit output).  image_rows_host NULL: image token i of the
+ * plan (n1_llm_plan_image_tokens of them, in plan order) reads feats[i]; n_rows must be 0 and feat_rows equal the image
+ * tokens, and feats may be NULL when there are none.  Otherwise feats is a feature pool and token i reads
+ * feats[image_rows_host[i]]: the HOST int32 table has one entry per image token, each a row of the pool (a row may serve
+ * several tokens).  The outputs are the same either way.
+ * eos_ids_host: <= 4 ids (Qwen2.5-VL generation config: 151645, 151643); a sequence stops after emitting one of them
+ * (the id is part of its output) or after max_new_tokens.  tokens_host [B, max_new_tokens] int32 (tail filled with
+ * pad_id), lens_host [B] = tokens emitted.  latents_bf16 (device, [B, n_query, 3584]) may be NULL.  *passes_host
+ * (nullable) = decode passes run.  The call synchronises `stream` (the stop test reads a device counter after every token).
+ * On a plan over a K/V pool the call refuses a reused length beyond the rows the slot holds (n1_kv_pool_valid), and
+ * afterwards the slot holds the prompt and every generated token whose K/V a pass wrote (all of them when latents_bf16
+ * is given, all but the last otherwise). */
+int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feats_bf16, int64_t feat_rows,
+                    const int32_t* image_rows_host, int64_t n_rows, const int32_t* eos_ids_host, int n_eos, int32_t pad_id,
+                    int32_t* tokens_host, int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
 
-/* ---- continuing a conversation on its K/V cache (the look-down turn of the policy)
- * A K/V pool is caller-owned device memory for `slots` conversations of up to `capacity` tokens each, in every decoder
- * layer: 2 * layers * kv_heads * head_dim * 2 bytes per token (57 344 B for Qwen2.5-VL-7B).  It is sized once.
- * n1_gen_plan_create_cont is n1_gen_plan_create over the FULL prompts and all their image grids, plus, per sequence, a
- * pool slot and the number of leading prompt tokens whose K/V that slot already holds (0: a fresh sequence, written to
- * the slot).  Only the remaining rows are embedded and prefilled, so image_feats covers only the images after that
- * prefix; the prefix may not end inside an image, the slots of one batch must differ, and prompt + max_new_tokens +
- * n_query must fit the capacity.  n1_llm_generate_pool is n1_llm_generate on such a plan; it refuses a reused length
- * beyond the rows the slot holds (n1_kv_pool_valid), and afterwards the slot holds the prompt and every generated token
- * whose K/V a pass wrote (all of them when latents_bf16 is given, all but the last otherwise). */
-typedef struct n1_kv_pool_s* n1_kv_pool;
+/* ---- K/V pool: caller-owned device memory for `slots` conversations of up to `capacity` tokens each, in every decoder
+ * layer: 2 * layers * kv_heads * head_dim * 2 bytes per token (57 344 B for Qwen2.5-VL-7B).  It is sized once, and a
+ * generation plan created over it continues the conversations its slots hold (the look-down turn of the policy). */
 int n1_kv_pool_create(n1_handle h, int slots, int capacity, n1_kv_pool* out);
 void n1_kv_pool_destroy(n1_kv_pool p);
 size_t n1_kv_pool_bytes(n1_kv_pool p);
 int n1_kv_pool_valid(n1_kv_pool p, int slot); /* rows slot holds, or a negative error code */
 /* copies rows [row, row + n) of a slot in one layer to DEVICE buffers k_out / v_out [n, kv_heads * head_dim] bf16 */
 int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_out, void* v_out, void* stream);
-int n1_gen_plan_create_cont(n1_handle h, const int32_t* input_ids_host, const int32_t* lens_host, int B,
-                            const int32_t* grid_thw_host, int n_img, int max_new_tokens, n1_kv_pool pool,
-                            const int32_t* reused_host, const int32_t* slots_host, n1_llm_plan* out, void* stream);
-int n1_llm_generate_pool(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes,
-                         const void* image_feats_bf16, const int32_t* eos_ids_host, int n_eos, int32_t pad_id,
-                         int32_t* tokens_host, int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
 /* content digest of n_img images, image i = rows [row_off[i], row_off[i + 1]) of bf16 pixels [*, cols] (all DEVICE
  * pointers; cols even) -> digest[i]: equal rows give equal digests, different rows differ with ~2^-64 odds */
 int n1_image_digest(const void* pixels_bf16, int64_t cols, const int64_t* row_off_dev, int n_img, uint64_t* digest_dev,
                     void* stream);
 
-/* ---- vision features kept across calls in a caller-owned feature pool: bf16 [pool_rows, 3584] (DEVICE)
- * Row tables are HOST int32 arrays; every entry must be a row of the pool, and each call checks that before it runs.
- * n1_qwen_vit_rows is n1_qwen_vit writing merged row r (original token order) to feat_pool[dst_rows_host[r]] instead of
- * out[r]; n_rows must equal n_patches / 4 and no row may appear twice.  No other pool row is written.
- * n1_llm_generate_rows / n1_llm_generate_pool_rows are n1_llm_generate / n1_llm_generate_pool with image token i of the
- * plan (n1_llm_plan_image_tokens of them, in plan order) read from feat_pool[image_rows_host[i]]; a row may serve several
- * tokens of one call.  The outputs equal those of the plain entry points on the gathered features. */
-int n1_qwen_vit_rows(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels_bf16, void* feat_pool_bf16,
-                     int64_t pool_rows, const int32_t* dst_rows_host, int64_t n_rows, void* stream);
-int n1_llm_generate_rows(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feat_pool_bf16,
-                         int64_t pool_rows, const int32_t* image_rows_host, int64_t n_rows, const int32_t* eos_ids_host,
-                         int n_eos, int32_t pad_id, int32_t* tokens_host, int32_t* lens_host, void* latents_bf16,
-                         int32_t* passes_host, void* stream);
-int n1_llm_generate_pool_rows(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes,
-                              const void* feat_pool_bf16, int64_t pool_rows, const int32_t* image_rows_host, int64_t n_rows,
-                              const int32_t* eos_ids_host, int n_eos, int32_t pad_id, int32_t* tokens_host,
-                              int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
-
 /* HOST-only integer helpers (no GPU needed): the same planners, exposed for bit-exact parity tests. */
 int n1_rope_index(const int32_t* input_ids_host, int len, const int32_t* grid_thw_host, int n_img, int merge,
                   int32_t* pos3_host /* [3, len] */, int32_t* delta_host);
-/* the row bookkeeping of a generation plan (n1_gen_plan_create, or n1_gen_plan_create_cont when reused_host / slots_host
- * are given with a pool of pool_slots x pool_capacity rows), without a device: *n_rows planned rows, cu_host [B + 1],
+/* the row bookkeeping of a generation plan (n1_llm_plan_create with max_new_tokens >= 1, over a pool of pool_slots x
+ * pool_capacity rows when reused_host / slots_host are given), without a device: *n_rows planned rows, cu_host [B + 1],
  * kind_host / src_host / dest_host [rows] (0 text / 1 image / 2 latent query, token id / feature row, K/V cache row),
  * k_len_host [B] keys after the prefill.  Row arrays hold at most cap_rows entries. */
 int n1_plan_rows_host(const int32_t* input_ids_host, const int32_t* lens_host, int B, const int32_t* grid_thw_host,
@@ -312,7 +295,7 @@ int n1_vl_patchify(const n1_vl_image* images_host, int n_img, const void* lut_bf
 size_t n1_rgb_tokens_workspace_bytes(n1_handle h, int B);
 int n1_rgb_tokens(n1_handle h, void* ws, size_t ws_bytes, const float* rgb, void* mem_bf16, int B, void* stream);
 /* Training branch, System-2 half (internvla_n1.py L128-235 and its backward): `plan` is a generation plan over the
- * prompts WITHOUT the TRAJ tokens (n1_gen_plan_create, max_new_tokens = 1).  Forward: states bf16 [B, n_query, hidden] =
+ * prompts WITHOUT the TRAJ tokens (n1_llm_plan_create, max_new_tokens = 1).  Forward: states bf16 [B, n_query, hidden] =
  * hidden states at the TRAJ positions.  Backward: grad_states bf16 [B, n_query, hidden] -> grad_latent_queries fp32
  * [n_query, hidden].  Both calls must be given the SAME workspace (the forward leaves its K/V cache and saves there). */
 int n1_s2_set_latent_queries(n1_handle h, const void* latent_queries_bf16, void* stream);  /* after an optimizer step */
@@ -433,7 +416,7 @@ int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int
 /* Chunk attention over a slotted K/V cache, head_dim 128 (wgmma): sequence b's query rows [cu_q[b], cu_q[b + 1]) of q are
  * its tokens ctx[b] .. ctx[b] + n_b - 1 and attend (bottom-right causal) to keys / values at rows row0[b] ..
  * row0[b] + ctx[b] + n_b - 1 of k / v ([kv_rows, heads_kv * 128], stride ldkv), which already hold the chunk's own K/V.
- * cu_q / ctx / row0 int32 on the device.  The continuation prefill of n1_llm_generate_pool runs it. */
+ * cu_q / ctx / row0 int32 on the device.  The prefill of n1_llm_generate on a plan over a K/V pool runs it. */
 int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
                           void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
                           int max_chunk, int heads_q, int heads_kv, float scale, void* stream);

@@ -3,45 +3,11 @@
 Validated on the H100 against PyTorch autograd / torch.optim (tests/test_bwd_ops_gpu.py);
 used by the training step (train_s1.py, train_step.py).  Nothing on the inference path imports this module.
 """
-import ctypes
-from ctypes import c_float, c_int, c_int64, c_void_p
+from ctypes import c_void_p
 
 import torch
 
-from . import _lib
-from ._lib import check, ptr, stream_ptr
-
-_bound = False
-BWD_SYMBOLS = ["n1_op_act_fwd", "n1_op_transpose", "n1_op_colsum", "n1_op_norm_bwd", "n1_op_act_bwd", "n1_op_swiglu_bwd",
-               "n1_op_rope_transposed", "n1_op_attention_bwd", "n1_op_adamw", "n1_op_sgemm", "n1_op_scale_cols",
-               "n1_op_patchify_depth", "n1_op_wgrad"]
-
-
-def _L():
-    global _bound
-    L = _lib.lib()
-    if not _bound:
-        vp = c_void_p
-        L.n1_op_transpose.argtypes = [vp, c_int, c_int, c_int, vp, c_int, c_int, vp]
-        L.n1_op_colsum.argtypes = [vp, vp, c_int, c_int, c_int, c_int, vp, c_int, vp]
-        L.n1_op_norm_bwd.argtypes = [vp, c_int, vp, c_int, vp, vp, c_int, vp, c_int, vp, vp, c_int, c_int, c_float, c_int,
-                                     c_int, vp]
-        L.n1_op_act_fwd.argtypes = [vp, vp, c_int64, c_int, vp]
-        L.n1_op_act_bwd.argtypes = [vp, vp, vp, c_int64, c_int, vp]
-        L.n1_op_swiglu_bwd.argtypes = [vp, vp, vp, c_int64, c_int, vp]
-        L.n1_op_rope_transposed.argtypes = [vp, c_int, vp, c_int64, c_int, c_int, vp]
-        L.n1_op_attention_bwd.argtypes = [vp] * 8 + [c_int] * 12 + [vp, vp, c_int, c_int, c_int, c_float, vp, c_int, vp]
-        L.n1_op_adamw.argtypes = [vp, vp, vp, vp, vp, c_int64, c_float, c_float, c_float, c_float, c_float, c_int, vp]
-        L.n1_op_sgemm.argtypes = [vp, c_int, c_int, vp, c_int, c_int, vp, c_int, c_int, c_int, c_int, c_int, vp]
-        L.n1_op_scale_cols.argtypes = [vp, c_int, vp, vp, c_int, vp, c_int, c_int64, c_int, vp]
-        L.n1_op_patchify_depth.argtypes = [vp, vp, c_int, c_int, vp]
-        L.n1_op_wgrad.argtypes = [vp, c_int, vp, c_int, c_int, c_int, c_int, vp, c_int, vp, ctypes.c_size_t, vp]
-        L.n1_op_wgrad_workspace_bytes.argtypes = [c_int, c_int, c_int]
-        L.n1_op_wgrad_workspace_bytes.restype = ctypes.c_size_t
-        for n in BWD_SYMBOLS:
-            getattr(L, n).restype = c_int
-        _bound = True
-    return L
+from ._lib import check, lib, ptr, stream_ptr
 
 
 def transpose(x, rows_pad=None):
@@ -49,7 +15,7 @@ def transpose(x, rows_pad=None):
     rows, cols = x.shape
     rows_pad = rows_pad or (rows + 7) // 8 * 8
     out = torch.empty(cols, rows_pad, dtype=torch.bfloat16, device=x.device)
-    check(_L().n1_op_transpose(ptr(x), rows, cols, x.stride(0), ptr(out), rows_pad, rows_pad, stream_ptr()))
+    check(lib().n1_op_transpose(ptr(x), rows, cols, x.stride(0), ptr(out), rows_pad, rows_pad, stream_ptr()))
     return out
 
 
@@ -57,8 +23,8 @@ def colsum(a, b=None, out=None, accumulate=False):
     rows, cols = a.shape
     if out is None:
         out = torch.zeros(cols, dtype=torch.float32, device=a.device)
-    check(_L().n1_op_colsum(ptr(a), ptr(b), rows, cols, a.stride(0), b.stride(0) if b is not None else 0, ptr(out),
-                            1 if accumulate else 0, stream_ptr()))
+    check(lib().n1_op_colsum(ptr(a), ptr(b), rows, cols, a.stride(0), b.stride(0) if b is not None else 0, ptr(out),
+                             1 if accumulate else 0, stream_ptr()))
     return out
 
 
@@ -67,33 +33,33 @@ def norm_bwd(dy, x, w, eps, rms=False, residual_grad=None, need_param_grads=True
     dx = torch.empty_like(x)
     dw = torch.zeros(D, dtype=torch.float32, device=x.device) if need_param_grads else None
     db = torch.zeros(D, dtype=torch.float32, device=x.device) if need_param_grads and not rms else None
-    check(_L().n1_op_norm_bwd(ptr(dy), dy.stride(0), ptr(x), x.stride(0), ptr(w), ptr(residual_grad),
-                              residual_grad.stride(0) if residual_grad is not None else 0, ptr(dx), dx.stride(0), ptr(dw),
-                              ptr(db), rows, D, eps, 1 if rms else 0, 0, stream_ptr()))
+    check(lib().n1_op_norm_bwd(ptr(dy), dy.stride(0), ptr(x), x.stride(0), ptr(w), ptr(residual_grad),
+                               residual_grad.stride(0) if residual_grad is not None else 0, ptr(dx), dx.stride(0), ptr(dw),
+                               ptr(db), rows, D, eps, 1 if rms else 0, 0, stream_ptr()))
     return dx, dw, db
 
 
 def act_fwd(pre, act):
     out = torch.empty_like(pre)
-    check(_L().n1_op_act_fwd(ptr(pre), ptr(out), pre.numel(), act, stream_ptr()))
+    check(lib().n1_op_act_fwd(ptr(pre), ptr(out), pre.numel(), act, stream_ptr()))
     return out
 
 
 def act_bwd(pre, dy, act):
     out = torch.empty_like(pre)
-    check(_L().n1_op_act_bwd(ptr(pre), ptr(dy), ptr(out), pre.numel(), act, stream_ptr()))
+    check(lib().n1_op_act_bwd(ptr(pre), ptr(dy), ptr(out), pre.numel(), act, stream_ptr()))
     return out
 
 
 def swiglu_bwd(pre, dact):
     out = torch.empty_like(pre)
-    check(_L().n1_op_swiglu_bwd(ptr(pre), ptr(dact), ptr(out), dact.shape[0], dact.shape[1], stream_ptr()))
+    check(lib().n1_op_swiglu_bwd(ptr(pre), ptr(dact), ptr(out), dact.shape[0], dact.shape[1], stream_ptr()))
     return out
 
 
 def rope_transposed(x, cos_sin, heads, head_dim):
     """in place on the first `heads` heads of every row of x [rows, >= heads * head_dim]; cos_sin fp32 [rows, hd/2, 2]"""
-    check(_L().n1_op_rope_transposed(ptr(x), x.stride(0), ptr(cos_sin), x.shape[0], heads, head_dim, stream_ptr()))
+    check(lib().n1_op_rope_transposed(ptr(x), x.stride(0), ptr(cos_sin), x.shape[0], heads, head_dim, stream_ptr()))
     return x
 
 
@@ -106,10 +72,10 @@ def attention_bwd(q, k, v, o, dout, heads_q, heads_kv, head_dim, batch, seq_q, s
     for t in (q, k, v, o, dout):   # column slices of packed projections are legal operands: row stride + unit inner stride
         assert t.is_cuda and t.dtype == torch.bfloat16 and t.stride(1) == 1
     vp = lambda t: c_void_p(t.data_ptr())
-    check(_L().n1_op_attention_bwd(vp(q), vp(k), vp(v), vp(o), vp(dout), ptr(dq), ptr(dk), ptr(dv), q.stride(0),
-                                   k.stride(0), v.stride(0), o.stride(0), dout.stride(0), dq.stride(0), heads_q, heads_kv,
-                                   head_dim, batch, seq_q, seq_k, ptr(cu_q), ptr(cu_k), max_seq_q, kv_div,
-                                   1 if causal else 0, scale, ptr(k_len), k_slot, stream_ptr()))
+    check(lib().n1_op_attention_bwd(vp(q), vp(k), vp(v), vp(o), vp(dout), ptr(dq), ptr(dk), ptr(dv), q.stride(0),
+                                    k.stride(0), v.stride(0), o.stride(0), dout.stride(0), dq.stride(0), heads_q, heads_kv,
+                                    head_dim, batch, seq_q, seq_k, ptr(cu_q), ptr(cu_k), max_seq_q, kv_div,
+                                    1 if causal else 0, scale, ptr(k_len), k_slot, stream_ptr()))
     return dq, dk, dv
 
 
@@ -132,7 +98,7 @@ def wgrad(dy, x, out=None, accumulate=False):
         assert not accumulate
         out = torch.empty(No, Ko, dtype=torch.float32, device=dy.device)
     assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (No, Ko)
-    L = _L()
+    L = lib()
     nb = L.n1_op_wgrad_workspace_bytes(M, No, Ko)
     ws = torch.empty(nb + 16, dtype=torch.uint8, device=dy.device)
     check(L.n1_op_wgrad(c_void_p(dy.data_ptr()), dy.stride(0), c_void_p(x.data_ptr()), x.stride(0), M, No, Ko, ptr(out),
@@ -149,8 +115,8 @@ def sgemm(a, b, trans_a=False, trans_b=False, out=None, accumulate=False):
     assert (b.shape[1] if trans_b else b.shape[0]) == K, (a.shape, b.shape, trans_a, trans_b)
     if out is None:
         out = torch.empty(M, N, dtype=torch.float32, device=a.device)
-    check(_L().n1_op_sgemm(c_void_p(a.data_ptr()), a.stride(0), 1 if trans_a else 0, c_void_p(b.data_ptr()), b.stride(0),
-                           1 if trans_b else 0, ptr(out), out.stride(0), M, N, K, 1 if accumulate else 0, stream_ptr()))
+    check(lib().n1_op_sgemm(c_void_p(a.data_ptr()), a.stride(0), 1 if trans_a else 0, c_void_p(b.data_ptr()), b.stride(0),
+                            1 if trans_b else 0, ptr(out), out.stride(0), M, N, K, 1 if accumulate else 0, stream_ptr()))
     return out
 
 
@@ -158,10 +124,10 @@ def scale_cols(x, gamma, add=None):
     """x [rows, cols] bf16 * gamma [cols] fp32 (+ add bf16) -> bf16."""
     assert x.dim() == 2 and x.stride(1) == 1 and x.dtype == torch.bfloat16 and gamma.dtype == torch.float32
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    check(_L().n1_op_scale_cols(c_void_p(x.data_ptr()), x.stride(0), ptr(gamma),
-                                c_void_p(add.data_ptr()) if add is not None else None,
-                                add.stride(0) if add is not None else 0, ptr(out), out.stride(0), x.shape[0], x.shape[1],
-                                stream_ptr()))
+    check(lib().n1_op_scale_cols(c_void_p(x.data_ptr()), x.stride(0), ptr(gamma),
+                                 c_void_p(add.data_ptr()) if add is not None else None,
+                                 add.stride(0) if add is not None else 0, ptr(out), out.stride(0), x.shape[0], x.shape[1],
+                                 stream_ptr()))
     return out
 
 
@@ -169,10 +135,10 @@ def patchify_depth(frames, ldk=200):
     """frames fp32 [n, 224, 224] -> bf16 [n * 256, ldk]: im2col of the 14 x 14 patches of one channel."""
     assert frames.dtype == torch.float32 and tuple(frames.shape[1:]) == (224, 224)
     out = torch.empty(frames.shape[0] * 256, ldk, dtype=torch.bfloat16, device=frames.device)
-    check(_L().n1_op_patchify_depth(ptr(frames), ptr(out), frames.shape[0], ldk, stream_ptr()))
+    check(lib().n1_op_patchify_depth(ptr(frames), ptr(out), frames.shape[0], ldk, stream_ptr()))
     return out
 
 
 def adamw(master, working, grad, m, v, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, step=1):
-    check(_L().n1_op_adamw(ptr(master), ptr(working), ptr(grad), ptr(m), ptr(v), master.numel(), lr, betas[0], betas[1], eps,
-                           weight_decay, step, stream_ptr()))
+    check(lib().n1_op_adamw(ptr(master), ptr(working), ptr(grad), ptr(m), ptr(v), master.numel(), lr, betas[0], betas[1], eps,
+                            weight_decay, step, stream_ptr()))

@@ -17,6 +17,8 @@ _lock = threading.Lock()
 
 c_void_p, c_int, c_size_t, c_float, c_char_p = (
     ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_float, ctypes.c_char_p)
+c_int32, c_int64, c_double = ctypes.c_int32, ctypes.c_int64, ctypes.c_double
+i32p = ctypes.POINTER(c_int32)
 
 
 class N1Error(RuntimeError):
@@ -36,6 +38,25 @@ class S1Dims(ctypes.Structure):
                 ("vlm_token_dim", ctypes.c_int32), ("n_query", ctypes.c_int32)]
 
 
+class NavdpPolicyDims(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("token_dim", "heads", "layers", "predict_size", "memory_size", "depth_frames",
+                                              "goal_slots", "ddpm_steps")]
+
+
+class S2Dims(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("v_depth", "v_hidden", "v_heads", "v_inter", "v_patch", "v_tpatch",
+                                              "v_merge", "v_window", "v_out", "n_fullatt")] + \
+               [("fullatt", ctypes.c_int32 * 16)] + \
+               [(n, ctypes.c_int32) for n in ("layers", "hidden", "heads", "kv_heads", "head_dim", "inter", "vocab")] + \
+               [("rms_eps", ctypes.c_float), ("rope_theta", ctypes.c_float), ("mrope", ctypes.c_int32 * 3),
+                ("n_query", ctypes.c_int32)]
+
+
+class VlImage(ctypes.Structure):
+    """n1_vl_image: one resized frame of n1_vl_patchify."""
+    _fields_ = [("src_u8", c_void_p), ("h", ctypes.c_int32), ("w", ctypes.c_int32), ("row0", ctypes.c_int64)]
+
+
 # every symbol include/n1b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "n1_version": (c_char_p, []),
@@ -51,7 +72,72 @@ SYMBOLS = {
                              c_int, c_int, c_int, c_void_p]),
     "n1_navdp_sample": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_int, c_int, c_int, c_int, c_void_p]),
+    "n1_navdp_policy_load": (c_int, [c_void_p, ctypes.POINTER(NavdpPolicyDims), ctypes.POINTER(TensorDesc), c_int,
+                                     c_void_p]),
+    "n1_navdp_critic": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "n1_ddpm_tables": (c_int, [c_int, ctypes.POINTER(c_float)]),
+    # System 2
+    "n1_s2_load": (c_int, [c_void_p, ctypes.POINTER(S2Dims), ctypes.POINTER(TensorDesc), c_int, c_void_p]),
+    "n1_s2_has_latent_queries": (c_int, [c_void_p]),
+    "n1_s2_has_lm_head": (c_int, [c_void_p]),
+    "n1_vit_plan_create": (c_int, [c_void_p, i32p, c_int, ctypes.POINTER(c_void_p), c_void_p]),
+    "n1_vit_plan_destroy": (None, [c_void_p]),
+    "n1_vit_plan_patches": (c_int64, [c_void_p]),
+    "n1_llm_plan_create": (c_int, [c_void_p, i32p, i32p, c_int, i32p, c_int, c_int, c_void_p, i32p, i32p,
+                                   ctypes.POINTER(c_void_p), c_void_p]),
+    "n1_llm_plan_destroy": (None, [c_void_p]),
+    "n1_llm_plan_tokens": (c_int64, [c_void_p]),
+    "n1_llm_plan_image_tokens": (c_int64, [c_void_p]),
+    "n1_llm_plan_positions": (c_int, [c_void_p, i32p, i32p]),
+    "n1_vit_workspace_bytes": (c_size_t, [c_void_p, c_void_p]),
+    "n1_llm_workspace_bytes": (c_size_t, [c_void_p, c_void_p]),
+    "n1_qwen_vit": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_int64, i32p, c_int64, c_void_p]),
+    "n1_llm_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "n1_llm_generate": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int64, i32p, c_int64, i32p, c_int,
+                                c_int32, i32p, i32p, c_void_p, i32p, c_void_p]),
+    "n1_kv_pool_create": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "n1_kv_pool_destroy": (None, [c_void_p]),
+    "n1_kv_pool_bytes": (c_size_t, [c_void_p]),
+    "n1_kv_pool_valid": (c_int, [c_void_p, c_int]),
+    "n1_kv_pool_read": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "n1_image_digest": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
+    "n1_rope_index": (c_int, [i32p, c_int, i32p, c_int, c_int, i32p, i32p]),
+    "n1_plan_rows_host": (c_int, [i32p, i32p, c_int, i32p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, i32p, i32p,
+                                  c_int, i32p, i32p, i32p, i32p, i32p, i32p]),
+    "n1_vit_window_index": (c_int, [i32p, c_int, c_int, c_int, i32p, i32p, i32p, i32p]),
+    "n1_s2_set_latent_queries": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "n1_s2_train_workspace_bytes": (c_size_t, [c_void_p, c_void_p]),
+    "n1_s2_train_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "n1_s2_train_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    # frame preprocessing and System-2 image rows
+    "n1_resize_plan_create": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p), c_void_p]),
+    "n1_resize_plan_destroy": (None, [c_void_p]),
+    "n1_resize_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int]),
+    "n1_resize_rgb_u8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "n1_resize_f32": (c_int, [c_void_p, c_void_p, c_int, c_float, c_float, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "n1_resize_coeffs": (c_int, [c_int, c_int, c_int, i32p, ctypes.POINTER(c_double), i32p, i32p]),
+    "n1_vl_patchify_workspace_bytes": (c_size_t, [c_int]),
+    "n1_vl_patchify": (c_int, [ctypes.POINTER(VlImage), c_int, c_void_p, c_void_p, c_int64, c_void_p, c_size_t, c_void_p]),
+    # training: backward primitives
+    "n1_op_transpose": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "n1_op_colsum": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "n1_op_norm_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                               c_void_p, c_int, c_int, c_float, c_int, c_int, c_void_p]),
+    "n1_op_act_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "n1_op_act_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "n1_op_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "n1_op_rope_transposed": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_void_p]),
+    "n1_op_attention_bwd": (c_int, [c_void_p] * 8 + [c_int] * 12 + [c_void_p, c_void_p, c_int, c_int, c_int, c_float,
+                                                                   c_void_p, c_int, c_void_p]),
+    "n1_op_sgemm": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                            c_void_p]),
+    "n1_op_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "n1_op_wgrad": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_size_t,
+                            c_void_p]),
+    "n1_op_scale_cols": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
+    "n1_op_patchify_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "n1_op_adamw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float, c_float,
+                            c_float, c_int, c_void_p]),
     "n1_rgb_tokens_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "n1_rgb_tokens": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]),
     "n1_traj_to_actions": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double, c_int, c_int, c_int,

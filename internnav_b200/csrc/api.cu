@@ -86,16 +86,23 @@ inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 inline const bf16* B16(const void* p) { return static_cast<const bf16*>(p); }
 inline bf16* B16(void* p) { return static_cast<bf16*>(p); }
 
-// A host row table into a feature pool of pool_rows rows: `expect` entries, each a row of the pool, and with `distinct`
-// no row twice (the rows a vision call writes).
+// The `expect` feature rows a call writes or reads in pool [pool_rows].  Without a host row table (rows NULL) they are
+// rows 0 .. expect - 1 of a buffer of exactly that many rows.  Otherwise the table has `expect` entries, each a row of
+// the pool, and with `distinct` no row twice (the rows a vision call writes).
 void check_rows(const char* fn, const void* pool, int64_t pool_rows, const int32_t* rows, int64_t n_rows, int64_t expect,
                 bool distinct) {
   const std::string f(fn);
+  if (!rows) {
+    if (n_rows != 0 || pool_rows != expect)
+      throw Error(N1_ERR_ARG, f + ": without a row table n_rows must be 0 and the features " + std::to_string(expect) +
+                                  " rows, got " + std::to_string(n_rows) + " and " + std::to_string(pool_rows));
+    if (expect > 0 && !pool) throw Error(N1_ERR_ARG, f + ": null features");
+    return;
+  }
   if (!pool || pool_rows <= 0 || pool_rows > INT32_MAX) throw Error(N1_ERR_ARG, f + ": null feature pool or bad pool_rows");
   if (n_rows != expect)
     throw Error(N1_ERR_ARG, f + ": the row table has " + std::to_string(n_rows) + " entries, the plan needs " +
                                 std::to_string(expect));
-  if (n_rows > 0 && !rows) throw Error(N1_ERR_ARG, f + ": null row table");
   std::vector<char> seen(distinct ? (size_t)pool_rows : 0, 0);
   for (int64_t i = 0; i < n_rows; ++i) {
     if (rows[i] < 0 || rows[i] >= pool_rows)
@@ -268,13 +275,15 @@ void n1_vit_plan_destroy(n1_vit_plan p) {
 int64_t n1_vit_plan_patches(n1_vit_plan p) { return p ? p->p->host.n_patches : 0; }
 
 int n1_llm_plan_create(n1_handle h, const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
-                       n1_llm_plan* out, void* stream) {
+                       int max_new_tokens, n1_kv_pool pool, const int32_t* reused, const int32_t* slots, n1_llm_plan* out,
+                       void* stream) {
   return guard([&] {
     use(h);
-    if (!ids || !lens || B <= 0 || !out) throw Error(N1_ERR_ARG, "n1_llm_plan_create: bad arguments");
+    if (!ids || !lens || B <= 0 || max_new_tokens < 0 || !out) throw Error(N1_ERR_ARG, "n1_llm_plan_create: bad arguments");
     n1_llm_plan_s* w = new n1_llm_plan_s();
     try {
-      w->p = h->s2.make_llm_plan(ids, lens, B, grid, n_img, S(stream));
+      w->p = h->s2.make_llm_plan(ids, lens, B, grid, n_img, S(stream), max_new_tokens, reused, slots,
+                                 pool ? pool->p : nullptr);
     } catch (...) {
       delete w;
       throw;
@@ -309,16 +318,20 @@ size_t n1_llm_workspace_bytes(n1_handle h, n1_llm_plan p) {
   size_t r = 0;
   guard([&] {
     if (!h || !p) throw Error(N1_ERR_ARG, "null handle/plan");
-    r = h->s2.ws_llm(*p->p);
+    r = p->p->max_new > 0 ? h->s2.ws_generate(*p->p) : h->s2.ws_llm(*p->p);
   });
   return r;
 }
 
-int n1_qwen_vit(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels, void* out, void* stream) {
+int n1_qwen_vit(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels, void* out, int64_t out_rows,
+                const int32_t* dst_rows, int64_t n_rows, void* stream) {
   return guard([&] {
+    if (!h || !p || !pixels) throw Error(N1_ERR_ARG, "n1_qwen_vit: null handle / plan / pixels");
+    const VitPlan& vp = *p->p;
+    const int unit = h->s2.dims.v_merge * h->s2.dims.v_merge;
+    check_rows("n1_qwen_vit", out, out_rows, dst_rows, n_rows, vp.host.n_patches / unit, true);
     use(h);
-    if (!p) throw Error(N1_ERR_ARG, "null plan");
-    h->s2.vit_forward(*p->p, ws, ws_bytes, B16(pixels), B16(out), S(stream));
+    h->s2.vit_forward(vp, ws, ws_bytes, B16(pixels), B16(out), S(stream), dst_rows);
   });
 }
 int n1_llm_prefill(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* image_feats, void* latents,
@@ -330,41 +343,19 @@ int n1_llm_prefill(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const 
   });
 }
 
-int n1_gen_plan_create(n1_handle h, const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
-                       int max_new_tokens, n1_llm_plan* out, void* stream) {
-  return guard([&] {
-    use(h);
-    if (!ids || !lens || B <= 0 || !out || max_new_tokens < 1) throw Error(N1_ERR_ARG, "n1_gen_plan_create: bad arguments");
-    n1_llm_plan_s* w = new n1_llm_plan_s();
-    try {
-      w->p = h->s2.make_llm_plan(ids, lens, B, grid, n_img, S(stream), max_new_tokens);
-    } catch (...) {
-      delete w;
-      throw;
-    }
-    *out = w;
-  });
-}
-size_t n1_generate_workspace_bytes(n1_handle h, n1_llm_plan p) {
-  size_t r = 0;
-  guard([&] {
-    if (!h || !p) throw Error(N1_ERR_ARG, "null handle/plan");
-    r = h->s2.ws_generate(*p->p);
-  });
-  return r;
-}
 int n1_s2_has_lm_head(n1_handle h) { return h && h->s2.has_lm_head() ? 1 : 0; }
 int n1_s2_has_latent_queries(n1_handle h) { return h && h->s2.has_latent_queries() ? 1 : 0; }
-int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* image_feats,
-                    const int32_t* eos, int n_eos, int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents,
-                    int32_t* passes, void* stream) {
+int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feats, int64_t feat_rows,
+                    const int32_t* image_rows, int64_t n_rows, const int32_t* eos, int n_eos, int32_t pad_id,
+                    int32_t* tokens, int32_t* lens, void* latents, int32_t* passes, void* stream) {
   return guard([&] {
-    use(h);
-    if (!p) throw Error(N1_ERR_ARG, "null plan");
+    if (!h || !p) throw Error(N1_ERR_ARG, "n1_llm_generate: null handle / plan");
     if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate: 0..4 eos ids");
+    check_rows("n1_llm_generate", feats, feat_rows, image_rows, n_rows, p->p->n_image_tokens, false);
+    use(h);
     GenResult r;
     r.tokens = tokens, r.lens = lens;
-    h->s2.llm_generate(*p->p, ws, ws_bytes, B16(image_feats), eos, n_eos, pad_id, r, B16(latents), S(stream));
+    h->s2.llm_generate(*p->p, ws, ws_bytes, B16(feats), eos, n_eos, pad_id, r, B16(latents), S(stream), image_rows);
     if (passes) *passes = r.steps;
   });
 }
@@ -410,84 +401,11 @@ int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_o
     N1_CUDA(cudaMemcpyAsync(v_out, q.v + off, (size_t)n * w * sizeof(bf16), cudaMemcpyDeviceToDevice, S(stream)));
   });
 }
-int n1_gen_plan_create_cont(n1_handle h, const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
-                            int max_new_tokens, n1_kv_pool pool, const int32_t* reused, const int32_t* slots,
-                            n1_llm_plan* out, void* stream) {
-  return guard([&] {
-    use(h);
-    if (!ids || !lens || B <= 0 || !out || max_new_tokens < 1 || !pool || !reused || !slots)
-      throw Error(N1_ERR_ARG, "n1_gen_plan_create_cont: bad arguments");
-    n1_llm_plan_s* w = new n1_llm_plan_s();
-    try {
-      w->p = h->s2.make_llm_plan(ids, lens, B, grid, n_img, S(stream), max_new_tokens, reused, slots, pool->p);
-    } catch (...) {
-      delete w;
-      throw;
-    }
-    *out = w;
-  });
-}
-int n1_llm_generate_pool(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes, const void* image_feats,
-                         const int32_t* eos, int n_eos, int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents,
-                         int32_t* passes, void* stream) {
-  return guard([&] {
-    use(h);
-    if (!p || !pool) throw Error(N1_ERR_ARG, "null plan / pool");
-    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_pool: 0..4 eos ids");
-    GenResult r;
-    r.tokens = tokens, r.lens = lens;
-    h->s2.llm_generate_pool(*p->p, *pool->p, ws, ws_bytes, B16(image_feats), eos, n_eos, pad_id, r, B16(latents),
-                            S(stream));
-    if (passes) *passes = r.steps;
-  });
-}
 int n1_image_digest(const void* pixels, int64_t cols, const int64_t* row_off, int n_img, uint64_t* digest, void* stream) {
   return guard([&] {
     if ((n_img > 0 && (!pixels || !row_off || !digest)) || n_img < 0 || cols <= 0)
       throw Error(N1_ERR_ARG, "n1_image_digest: bad arguments");
     image_digest(B16(pixels), cols, row_off, n_img, digest, S(stream));
-  });
-}
-
-int n1_qwen_vit_rows(n1_handle h, n1_vit_plan p, void* ws, size_t ws_bytes, const void* pixels, void* feat_pool,
-                     int64_t pool_rows, const int32_t* dst_rows, int64_t n_rows, void* stream) {
-  return guard([&] {
-    if (!h || !p || !pixels) throw Error(N1_ERR_ARG, "n1_qwen_vit_rows: null handle / plan / pixels");
-    const VitPlan& vp = *p->p;
-    const int unit = h->s2.dims.v_merge * h->s2.dims.v_merge;
-    check_rows("n1_qwen_vit_rows", feat_pool, pool_rows, dst_rows, n_rows, vp.host.n_patches / unit, true);
-    use(h);
-    h->s2.vit_forward(vp, ws, ws_bytes, B16(pixels), B16(feat_pool), S(stream), dst_rows);
-  });
-}
-int n1_llm_generate_rows(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feat_pool, int64_t pool_rows,
-                         const int32_t* image_rows, int64_t n_rows, const int32_t* eos, int n_eos, int32_t pad_id,
-                         int32_t* tokens, int32_t* lens, void* latents, int32_t* passes, void* stream) {
-  return guard([&] {
-    if (!h || !p) throw Error(N1_ERR_ARG, "n1_llm_generate_rows: null handle / plan");
-    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_rows: 0..4 eos ids");
-    check_rows("n1_llm_generate_rows", feat_pool, pool_rows, image_rows, n_rows, p->p->n_image_tokens, false);
-    use(h);
-    GenResult r;
-    r.tokens = tokens, r.lens = lens;
-    h->s2.llm_generate(*p->p, ws, ws_bytes, B16(feat_pool), eos, n_eos, pad_id, r, B16(latents), S(stream), image_rows);
-    if (passes) *passes = r.steps;
-  });
-}
-int n1_llm_generate_pool_rows(n1_handle h, n1_llm_plan p, n1_kv_pool pool, void* ws, size_t ws_bytes, const void* feat_pool,
-                              int64_t pool_rows, const int32_t* image_rows, int64_t n_rows, const int32_t* eos, int n_eos,
-                              int32_t pad_id, int32_t* tokens, int32_t* lens, void* latents, int32_t* passes,
-                              void* stream) {
-  return guard([&] {
-    if (!h || !p || !pool) throw Error(N1_ERR_ARG, "n1_llm_generate_pool_rows: null handle / plan / pool");
-    if (n_eos < 0 || n_eos > 4 || (n_eos > 0 && !eos)) throw Error(N1_ERR_ARG, "n1_llm_generate_pool_rows: 0..4 eos ids");
-    check_rows("n1_llm_generate_pool_rows", feat_pool, pool_rows, image_rows, n_rows, p->p->n_image_tokens, false);
-    use(h);
-    GenResult r;
-    r.tokens = tokens, r.lens = lens;
-    h->s2.llm_generate_pool(*p->p, *pool->p, ws, ws_bytes, B16(feat_pool), eos, n_eos, pad_id, r, B16(latents),
-                            S(stream), image_rows);
-    if (passes) *passes = r.steps;
   });
 }
 

@@ -251,13 +251,13 @@ KvPool* S2Model::make_pool(int slots, int cap) const {
 
 LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img,
                                 cudaStream_t s, int max_new_tokens, const int32_t* ctx_in, const int32_t* slot_in,
-                                const KvPool* pool) const {
+                                KvPool* pool) const {
   N1_CHECK(loaded_, "System-2 weights not loaded");
-  N1_CHECK(max_new_tokens != 0, "generation plan: max_new_tokens must be >= 1");
+  N1_CHECK(max_new_tokens >= 0, "llm plan: max_new_tokens must be >= 0");
   const bool cont = pool != nullptr;
   N1_CHECK(cont == (ctx_in != nullptr) && cont == (slot_in != nullptr), "continuation plan: ctx, slots and pool go together");
   N1_CHECK(!cont || max_new_tokens > 0, "continuation plan: only generation plans continue a cache");
-  if (max_new_tokens < 0 && !has_latent_queries())
+  if (max_new_tokens == 0 && !has_latent_queries())
     throw Error(-6, "latent plan: its prompts end in TRAJ tokens, and latent_queries was not part of the loaded state_dict "
                     "(a System-2-only model)");
   std::unique_ptr<LlmPlan> p(new LlmPlan());
@@ -586,38 +586,26 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
                            const int32_t* image_rows_host) const {
   N1_CHECK(loaded_ && ws, "llm_generate: not loaded / null workspace");
   N1_CHECK(p.max_new > 0, "llm_generate: the plan was not created for generation");
-  N1_CHECK(!p.pool, "llm_generate: a continuation plan needs its K/V pool (n1_llm_generate_pool)");
   if (!has_lm_head()) throw Error(-6, "llm_generate: lm_head.weight was not part of the loaded state_dict");
   if (latents && !has_latent_queries())
     throw Error(-6, "llm_generate: latents requested, but latent_queries was not part of the loaded state_dict");
   N1_CHECK(out.tokens && out.lens, "llm_generate: null output buffers");
+  KvPool* pool = p.pool;
+  if (pool)
+    for (int b = 0; b < p.B; ++b)
+      N1_CHECK(p.h_ctx[b] <= pool->valid[p.h_slot[b]],
+               "llm_generate: sequence " + std::to_string(b) + " reuses " + std::to_string(p.h_ctx[b]) +
+                   " rows but slot " + std::to_string(p.h_slot[b]) + " holds " + std::to_string(pool->valid[p.h_slot[b]]));
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate: workspace too small");
-  p.wait_ready(s);
-  gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s, image_rows_host);
-  p.mark_used(s);
-}
-
-void S2Model::llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
-                                const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents,
-                                cudaStream_t s, const int32_t* image_rows_host) const {
-  N1_CHECK(loaded_ && ws, "llm_generate_pool: not loaded / null workspace");
-  N1_CHECK(p.pool == &pool, "llm_generate_pool: the plan was not created for this K/V pool");
-  if (!has_lm_head()) throw Error(-6, "llm_generate_pool: lm_head.weight was not part of the loaded state_dict");
-  if (latents && !has_latent_queries())
-    throw Error(-6, "llm_generate_pool: latents requested, but latent_queries was not part of the loaded state_dict");
-  N1_CHECK(out.tokens && out.lens, "llm_generate_pool: null output buffers");
-  for (int b = 0; b < p.B; ++b)
-    N1_CHECK(p.h_ctx[b] <= pool.valid[p.h_slot[b]],
-             "llm_generate_pool: sequence " + std::to_string(b) + " reuses " + std::to_string(p.h_ctx[b]) +
-                 " rows but slot " + std::to_string(p.h_slot[b]) + " holds " + std::to_string(pool.valid[p.h_slot[b]]));
-  if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate_pool: workspace too small");
-  for (int b = 0; b < p.B; ++b) pool.valid[p.h_slot[b]] = p.h_ctx[b];  // rows past ctx are rewritten from here on
+  if (pool)  // rows past ctx are rewritten from here on
+    for (int b = 0; b < p.B; ++b) pool->valid[p.h_slot[b]] = p.h_ctx[b];
   p.wait_ready(s);
   gen_impl(Carver(ws, ws_bytes), p, image_feats, eos, n_eos, pad, &out, latents, s, image_rows_host);
   p.mark_used(s);
   // K/V exist for the prompt and every generated token but the last; the latent pass writes the last one too (and the
   // TRAJ rows after it, which are not part of the conversation)
-  for (int b = 0; b < p.B; ++b) pool.valid[p.h_slot[b]] = p.h_len[b] + out.lens[b] - (latents ? 0 : 1);
+  if (pool)
+    for (int b = 0; b < p.B; ++b) pool->valid[p.h_slot[b]] = p.h_len[b] + out.lens[b] - (latents ? 0 : 1);
 }
 
 }  // namespace n1

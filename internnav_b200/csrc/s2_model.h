@@ -57,7 +57,7 @@ struct LlmPlan {
   int *dest_rows = nullptr, *d_len = nullptr, *d_delta = nullptr;  // [tokens], [B], [B]
   // continuation plans only (pool != nullptr): sequence b reuses the first ctx[b] rows of pool slot h_slot[b]; the plan's
   // rows are the suffix [ctx[b], len[b]) of each prompt, and its K/V live in the pool (first row row0[b])
-  const KvPool* pool = nullptr;
+  KvPool* pool = nullptr;
   std::vector<int> h_ctx, h_slot, h_len;
   int *ctx = nullptr, *row0 = nullptr;
   bool any_ctx = false;  // some sequence reuses rows: the prefill attends through the pool (attention_cache)
@@ -88,22 +88,22 @@ class S2Model {
   bool loaded() const { return loaded_; }
 
   VitPlan* make_vit_plan(const int32_t* grid_thw_host, int n_img, cudaStream_t s) const;
-  // ids: packed prompt token ids (host), lens[B]; TRAJ tokens are appended per sequence by the planner.
-  // max_new_tokens < 0: latent plan (generate_latents).  >= 1: generation plan (no TRAJ tokens; KV-cache slots sized
-  // for the prompt + max_new_tokens + n_query rows).
+  // ids: packed prompt token ids (host), lens[B].
+  // max_new_tokens 0: latent plan (generate_latents; TRAJ tokens are appended per sequence by the planner).  >= 1:
+  // generation plan (no TRAJ tokens; KV-cache slots sized for the prompt + max_new_tokens + n_query rows).
   // ctx_host / slot_host / pool (all or none; generation plans only): a continuation plan over the FULL prompts and all
   // their image grids (mRoPE positions come from the whole prompt) that embeds and prefills rows [ctx[b], len[b]) only;
   // image features are expected for the images whose tokens lie in those rows, and no image may straddle ctx[b].
   LlmPlan* make_llm_plan(const int32_t* ids_host, const int32_t* lens_host, int B, const int32_t* grid_thw_host,
-                         int n_img, cudaStream_t s, int max_new_tokens = -1, const int32_t* ctx_host = nullptr,
-                         const int32_t* slot_host = nullptr, const KvPool* pool = nullptr) const;
+                         int n_img, cudaStream_t s, int max_new_tokens, const int32_t* ctx_host, const int32_t* slot_host,
+                         KvPool* pool) const;
   KvPool* make_pool(int slots, int cap) const;
 
   size_t ws_vit(const VitPlan& p) const;
   // pixels bf16 [n_patches, 3 * tpatch * patch^2] -> out bf16 [n_patches / merge^2, v_out] (original token order).
   // dst_rows_host (host, n_patches / merge^2 entries, checked by the caller): merged row r goes to out[dst_rows_host[r]].
   void vit_forward(const VitPlan& p, void* ws, size_t ws_bytes, const bf16* pixels, bf16* out, cudaStream_t s,
-                   const int32_t* dst_rows_host = nullptr) const;
+                   const int32_t* dst_rows_host) const;
   size_t ws_llm(const LlmPlan& p) const;
   // image_feats bf16 [n_image_tokens, hidden] -> out bf16 [B, n_query, hidden] (final-norm states of the TRAJ rows)
   void llm_prefill(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, bf16* out,
@@ -114,14 +114,10 @@ class S2Model {
   // pass over [last token, TRAJ x n_query] per sequence -> latents bf16 [B, n_query, hidden].  Synchronises `s`.
   // image_rows_host (host, n_image_tokens entries, checked by the caller): image token i reads image_feats row
   // image_rows_host[i] instead of row i (image_feats is then a feature pool).
+  // On a continuation plan K/V are read from and written to the plan's pool, and pool->valid is updated.
   size_t ws_generate(const LlmPlan& p) const;
   void llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, const int32_t* eos, int n_eos,
-                    int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
-                    const int32_t* image_rows_host = nullptr) const;
-  // the same on a continuation plan: K/V are read from and written to `pool` (the plan's), and pool.valid is updated
-  void llm_generate_pool(const LlmPlan& p, KvPool& pool, void* ws, size_t ws_bytes, const bf16* image_feats,
-                         const int32_t* eos, int n_eos, int32_t pad, GenResult& out, bf16* latents, cudaStream_t s,
-                         const int32_t* image_rows_host = nullptr) const;
+                    int32_t pad, GenResult& out, bf16* latents, cudaStream_t s, const int32_t* image_rows_host) const;
   bool has_lm_head() const { return lm_head_.w != nullptr; }
   // optional ("model.latent_queries"); every call that embeds TRAJ rows needs it and refuses to run without it
   bool has_latent_queries() const { return latentq_ != nullptr; }

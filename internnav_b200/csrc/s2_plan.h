@@ -33,13 +33,13 @@ void rope_index_one(const int32_t* ids, int len, const int32_t* grid_thw, int n_
                     std::vector<int>& pos3, int& delta);
 
 // Token bookkeeping of one decoder plan over B packed prompts (all host integer work of S2Model::make_llm_plan).
-//   max_new < 0: latent plan (n_query TRAJ tokens appended per prompt); >= 1: generation plan, K/V rows of sequence b at
+//   max_new 0: latent plan (n_query TRAJ tokens appended per prompt); >= 1: generation plan, K/V rows of sequence b at
 //   b * slot + i with slot = max_len + max_new + n_query.
 //   ctx / slots (continuation plan, generation only): sequence b reuses the first ctx[b] rows of pool slot slots[b]
 //   (pool_slots x pool_cap rows); its rows are [ctx[b], len[b]) only, their K/V rows slots[b] * pool_cap + i, and image
 //   features are expected for the images after ctx[b] alone.
 struct PlanArgs {
-  int merge = 2, vocab = 0, n_query = 0, max_new = -1;
+  int merge = 2, vocab = 0, n_query = 0, max_new = 0;
   const int32_t* ctx = nullptr;
   const int32_t* slots = nullptr;
   int pool_slots = 0, pool_cap = 0;

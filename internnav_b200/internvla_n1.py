@@ -211,7 +211,7 @@ class InternVLAN1ForCausalLM:
         prompts are right-aligned the way the HF processor pads them (left padding).  Other HF keyword arguments
         (attention_mask, use_cache, ...) are accepted and have no effect on greedy search.  `past_key_values`: one KVCache
         (or None) per prompt, from `make_kv_pool(...).handle(slot)` or a previous call's `out.past_key_values`; the
-        longest reusable prefix of each prompt is then neither re-encoded nor re-prefilled (qwen.System2._generate_cached),
+        longest reusable prefix of each prompt is then neither re-encoded nor re-prefilled (qwen.System2.generate),
         and the output also carries `past_key_values` (one new KVCache per prompt), `prefill_rows` and `vit_patches`.
         A None entry next to KVCaches starts a fresh conversation on an unused slot of their pool; a list of None only
         (no pool to write to) is an uncached call.  `feature_pool` (from `make_feature_pool`): the vision tower runs only

@@ -14,13 +14,8 @@ import ctypes
 import torch
 
 from . import _bwd, _lib
-from ._lib import OP_DENOISE, OP_RGBD, TensorDesc, c_void_p, check
+from ._lib import OP_DENOISE, OP_RGBD, NavdpPolicyDims, TensorDesc, c_void_p, check
 from .navdp import NavDP_Policy_DPT_CriticSum_DAT
-
-
-class PolicyDims(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int32) for n in ("token_dim", "heads", "layers", "predict_size", "memory_size", "depth_frames",
-                                              "goal_slots", "ddpm_steps")]
 
 
 _RENAME = {
@@ -44,12 +39,6 @@ class NavDPNet(NavDP_Policy_DPT_CriticSum_DAT):
         dev = self._device
         if dev.type != "cuda":
             raise RuntimeError("n1b200 has no CPU path: construct NavDPNet with device='cuda:N'")
-        L.n1_navdp_policy_load.restype = ctypes.c_int
-        L.n1_navdp_policy_load.argtypes = [c_void_p, ctypes.POINTER(PolicyDims), ctypes.POINTER(TensorDesc), ctypes.c_int,
-                                           c_void_p]
-        L.n1_navdp_critic.restype = ctypes.c_int
-        L.n1_navdp_critic.argtypes = [c_void_p, c_void_p, ctypes.c_size_t, c_void_p, c_void_p, c_void_p, ctypes.c_int,
-                                      ctypes.c_int, ctypes.c_int, c_void_p]
         flat = {}
         for k, v in sd.items():
             if not torch.is_tensor(v) or not v.is_floating_point():
@@ -78,8 +67,8 @@ class NavDPNet(NavDP_Policy_DPT_CriticSum_DAT):
                 d.shape[i] = s
             descs.append(d)
         arr = (TensorDesc * len(descs))(*descs)
-        dims = PolicyDims(self.token_dim, self.attention_heads, self.temporal_depth, self.predict_size, self.memory_size, 1,
-                          3, self.num_train_timesteps)
+        dims = NavdpPolicyDims(self.token_dim, self.attention_heads, self.temporal_depth, self.predict_size,
+                               self.memory_size, 1, 3, self.num_train_timesteps)
         with torch.cuda.device(dev):
             check(L.n1_navdp_policy_load(h, ctypes.byref(dims), arr, len(descs), _lib.stream_ptr()))
             torch.cuda.synchronize()

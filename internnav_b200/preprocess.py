@@ -26,50 +26,14 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check
+from ._lib import VlImage, check
 
 SYS1_DEPTH_THRESHOLD = 5.0
-_bound = False
-
-
-def _bind(L):
-    global _bound
-    if _bound:
-        return
-    vp, ci = c_void_p, ctypes.c_int
-    L.n1_resize_plan_create.restype = ci
-    L.n1_resize_plan_create.argtypes = [ci, ci, ci, ci, ctypes.POINTER(vp), vp]
-    L.n1_resize_plan_destroy.restype = None
-    L.n1_resize_plan_destroy.argtypes = [vp]
-    L.n1_resize_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_resize_workspace_bytes.argtypes = [vp, ci, ci]
-    L.n1_resize_rgb_u8.restype = ci
-    L.n1_resize_rgb_u8.argtypes = [vp, vp, ci, vp, vp, vp, ctypes.c_size_t, vp]
-    L.n1_resize_f32.restype = ci
-    L.n1_resize_f32.argtypes = [vp, vp, ci, ctypes.c_float, ctypes.c_float, vp, vp, ctypes.c_size_t, vp]
-    L.n1_resize_coeffs.restype = ci
-    L.n1_resize_coeffs.argtypes = [ci, ci, ci, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double),
-                                   ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]
-    L.n1_vl_patchify_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_vl_patchify_workspace_bytes.argtypes = [ci]
-    L.n1_vl_patchify.restype = ci
-    L.n1_vl_patchify.argtypes = [ctypes.POINTER(VlImage), ci, vp, vp, ctypes.c_int64, vp, ctypes.c_size_t, vp]
-    _bound = True
-
-
-class VlImage(ctypes.Structure):
-    """n1_vl_image: one resized frame of n1_vl_patchify."""
-    _fields_ = [("src_u8", c_void_p), ("h", ctypes.c_int32), ("w", ctypes.c_int32), ("row0", ctypes.c_int64)]
-
-
-RESIZE_SYMBOLS = ["n1_resize_plan_create", "n1_resize_plan_destroy", "n1_resize_workspace_bytes", "n1_resize_rgb_u8",
-                  "n1_resize_f32", "n1_resize_coeffs", "n1_vl_patchify_workspace_bytes", "n1_vl_patchify"]
 
 
 def resize_coeffs(in_size, out_size):
     """Host-only: Pillow's per-axis tables as computed by the library -> (bounds [out,2], weights [out,k], fixed [out,k])."""
     L = _lib.lib()
-    _bind(L)
     cap = 4 * max(1, -(-in_size // out_size)) + 8
     b = (ctypes.c_int32 * (out_size * 2))()
     w = (ctypes.c_double * (out_size * cap))()
@@ -87,7 +51,6 @@ class _ResizePlans:
 
     def __init__(self, device):
         self.device, self._plans = device, {}
-        _bind(_lib.lib())
 
     def __del__(self):
         try:

@@ -12,22 +12,13 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import TensorDesc, c_void_p, check
+from ._lib import S2Dims, TensorDesc, c_void_p, check
 
 QWEN25VL_7B = dict(
     v_depth=32, v_hidden=1280, v_heads=16, v_inter=3420, v_patch=14, v_tpatch=2, v_merge=2, v_window=112, v_out=3584,
     fullatt=[7, 15, 23, 31],
     layers=28, hidden=3584, heads=28, kv_heads=4, head_dim=128, inter=18944, vocab=152064,
     rms_eps=1e-6, rope_theta=1000000.0, mrope=[16, 24, 24], n_query=4)
-
-
-class S2Dims(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int32) for n in ("v_depth", "v_hidden", "v_heads", "v_inter", "v_patch", "v_tpatch",
-                                              "v_merge", "v_window", "v_out", "n_fullatt")] + \
-               [("fullatt", ctypes.c_int32 * 16)] + \
-               [(n, ctypes.c_int32) for n in ("layers", "hidden", "heads", "kv_heads", "head_dim", "inter", "vocab")] + \
-               [("rms_eps", ctypes.c_float), ("rope_theta", ctypes.c_float), ("mrope", ctypes.c_int32 * 3),
-                ("n_query", ctypes.c_int32)]
 
 
 def _dims_struct(cfg):
@@ -43,108 +34,6 @@ def _dims_struct(cfg):
         d.mrope[i] = int(cfg["mrope"][i])
     return d
 
-
-def _bind(L):
-    if getattr(L, "_s2_bound", False):
-        return
-    vp = c_void_p
-    L.n1_s2_load.restype = ctypes.c_int
-    L.n1_s2_load.argtypes = [vp, ctypes.POINTER(S2Dims), ctypes.POINTER(TensorDesc), ctypes.c_int, vp]
-    L.n1_vit_plan_create.restype = ctypes.c_int
-    L.n1_vit_plan_create.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.POINTER(vp), vp]
-    L.n1_vit_plan_destroy.restype = None
-    L.n1_vit_plan_destroy.argtypes = [vp]
-    L.n1_vit_plan_patches.restype = ctypes.c_int64
-    L.n1_vit_plan_patches.argtypes = [vp]
-    L.n1_llm_plan_create.restype = ctypes.c_int
-    L.n1_llm_plan_create.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
-                                     ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.POINTER(vp), vp]
-    L.n1_llm_plan_destroy.restype = None
-    L.n1_llm_plan_destroy.argtypes = [vp]
-    L.n1_llm_plan_tokens.restype = ctypes.c_int64
-    L.n1_llm_plan_tokens.argtypes = [vp]
-    L.n1_llm_plan_image_tokens.restype = ctypes.c_int64
-    L.n1_llm_plan_image_tokens.argtypes = [vp]
-    L.n1_llm_plan_positions.restype = ctypes.c_int
-    L.n1_llm_plan_positions.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]
-    L.n1_vit_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_vit_workspace_bytes.argtypes = [vp, vp]
-    L.n1_llm_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_llm_workspace_bytes.argtypes = [vp, vp]
-    L.n1_qwen_vit.restype = ctypes.c_int
-    L.n1_qwen_vit.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
-    L.n1_llm_prefill.restype = ctypes.c_int
-    L.n1_llm_prefill.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
-    L.n1_rope_index.restype = ctypes.c_int
-    L.n1_vit_window_index.restype = ctypes.c_int
-    L.n1_gen_plan_create.restype = ctypes.c_int
-    L.n1_gen_plan_create.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
-                                     ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp), vp]
-    L.n1_generate_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_generate_workspace_bytes.argtypes = [vp, vp]
-    L.n1_s2_has_lm_head.restype = ctypes.c_int
-    L.n1_s2_has_lm_head.argtypes = [vp]
-    L.n1_s2_has_latent_queries.restype = ctypes.c_int
-    L.n1_s2_has_latent_queries.argtypes = [vp]
-    L.n1_llm_generate.restype = ctypes.c_int
-    L.n1_llm_generate.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
-                                  ctypes.c_int32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
-                                  ctypes.POINTER(ctypes.c_int32), vp]
-    L.n1_s2_set_latent_queries.restype = ctypes.c_int
-    L.n1_s2_set_latent_queries.argtypes = [vp, vp, vp]
-    L.n1_s2_train_workspace_bytes.restype = ctypes.c_size_t
-    L.n1_s2_train_workspace_bytes.argtypes = [vp, vp]
-    L.n1_s2_train_forward.restype = ctypes.c_int
-    L.n1_s2_train_forward.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
-    L.n1_s2_train_backward.restype = ctypes.c_int
-    L.n1_s2_train_backward.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, vp]
-    L.n1_kv_pool_create.restype = ctypes.c_int
-    L.n1_kv_pool_create.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]
-    L.n1_kv_pool_destroy.restype = None
-    L.n1_kv_pool_destroy.argtypes = [vp]
-    L.n1_kv_pool_bytes.restype = ctypes.c_size_t
-    L.n1_kv_pool_bytes.argtypes = [vp]
-    L.n1_kv_pool_valid.restype = ctypes.c_int
-    L.n1_kv_pool_valid.argtypes = [vp, ctypes.c_int]
-    L.n1_kv_pool_read.restype = ctypes.c_int
-    L.n1_kv_pool_read.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp]
-    i32p = ctypes.POINTER(ctypes.c_int32)
-    L.n1_plan_rows_host.restype = ctypes.c_int
-    L.n1_plan_rows_host.argtypes = [i32p, i32p, ctypes.c_int, i32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, i32p, i32p, ctypes.c_int, i32p, i32p, i32p,
-                                    i32p, i32p, i32p]
-    L.n1_gen_plan_create_cont.restype = ctypes.c_int
-    L.n1_gen_plan_create_cont.argtypes = [vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
-                                          ctypes.POINTER(ctypes.c_int32), ctypes.c_int, ctypes.c_int, vp,
-                                          ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(vp),
-                                          vp]
-    L.n1_llm_generate_pool.restype = ctypes.c_int
-    L.n1_llm_generate_pool.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp, ctypes.POINTER(ctypes.c_int32), ctypes.c_int,
-                                       ctypes.c_int32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
-                                       ctypes.POINTER(ctypes.c_int32), vp]
-    L.n1_image_digest.restype = ctypes.c_int
-    L.n1_image_digest.argtypes = [vp, ctypes.c_int64, vp, ctypes.c_int, vp, vp]
-    i64 = ctypes.c_int64
-    L.n1_qwen_vit_rows.restype = ctypes.c_int
-    L.n1_qwen_vit_rows.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, vp, i64, i32p, i64, vp]
-    L.n1_llm_generate_rows.restype = ctypes.c_int
-    L.n1_llm_generate_rows.argtypes = [vp, vp, vp, ctypes.c_size_t, vp, i64, i32p, i64, i32p, ctypes.c_int,
-                                       ctypes.c_int32, i32p, i32p, vp, i32p, vp]
-    L.n1_llm_generate_pool_rows.restype = ctypes.c_int
-    L.n1_llm_generate_pool_rows.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp, i64, i32p, i64, i32p, ctypes.c_int,
-                                            ctypes.c_int32, i32p, i32p, vp, i32p, vp]
-    L._s2_bound = True
-
-
-S2_SYMBOLS = ["n1_s2_load", "n1_vit_plan_create", "n1_vit_plan_destroy", "n1_vit_plan_patches", "n1_llm_plan_create",
-              "n1_llm_plan_destroy", "n1_llm_plan_tokens", "n1_llm_plan_image_tokens", "n1_llm_plan_positions",
-              "n1_vit_workspace_bytes", "n1_llm_workspace_bytes", "n1_qwen_vit", "n1_llm_prefill", "n1_rope_index",
-              "n1_vit_window_index", "n1_gen_plan_create", "n1_generate_workspace_bytes", "n1_s2_has_lm_head",
-              "n1_s2_has_latent_queries",
-              "n1_llm_generate", "n1_s2_train_workspace_bytes", "n1_s2_train_forward", "n1_s2_train_backward", "n1_s2_set_latent_queries",
-              "n1_kv_pool_create", "n1_kv_pool_destroy", "n1_kv_pool_bytes", "n1_kv_pool_valid", "n1_kv_pool_read", "n1_plan_rows_host", "n1_gen_plan_create_cont",
-              "n1_llm_generate_pool", "n1_image_digest", "n1_qwen_vit_rows", "n1_llm_generate_rows",
-              "n1_llm_generate_pool_rows"]
 
 EOS_TOKEN_IDS = (151645, 151643)  # Qwen2.5-VL generation_config.json: <|im_end|>, <|endoftext|>
 PAD_TOKEN_ID = 151643
@@ -230,7 +119,6 @@ class KVPool:
 
     def __init__(self, s2, slots, capacity):
         L = _lib.lib()
-        _bind(L)
         self.s2, self.slots, self.capacity = s2, int(slots), int(capacity)
         h = c_void_p()
         with torch.cuda.device(s2.device):
@@ -349,7 +237,6 @@ class System2:
     # ------------------------------------------------------------------ weights
     def load_state_dict(self, state_dict):
         L = _lib.lib()
-        _bind(L)
         dev = self.device
         if dev.type != "cuda":
             raise RuntimeError("n1b200 has no CPU path: System2 needs device='cuda:N'")
@@ -381,7 +268,7 @@ class System2:
             for p in self._vit_plans.values():
                 L.n1_vit_plan_destroy(p)
             for p in self._llm_plans.values():
-                L.n1_llm_plan_destroy(p[0])
+                L.n1_llm_plan_destroy(p)
             if self._handle is not None:
                 L.n1_destroy(self._handle)
         except Exception:
@@ -418,25 +305,30 @@ class System2:
             self._vit_plans[key] = p
         return p
 
-    def llm_plan(self, prompts, grid_thw):
-        """prompts: list of token-id lists (no TRAJ tokens); grid_thw: image grids in prompt order across the batch."""
+    def llm_plan(self, prompts, grid_thw, max_new_tokens=0, pool=None, reused=None, slots=None):
+        """Decoder plan, cached by its arguments.  prompts: list of token-id lists (no TRAJ tokens); grid_thw: image grids
+        in prompt order across the batch.  max_new_tokens 0: a latent plan (prefill_latents); >= 1: a generation plan,
+        which with a KVPool `pool` continues sequence b on slot slots[b], whose first reused[b] tokens it reuses."""
         gkey = tuple(int(v) for g in grid_thw for v in g)
-        key = (tuple(tuple(p) for p in prompts), gkey)
-        hit = self._llm_plans.get(key)
-        if hit is None:
+        cont = None if pool is None else (pool.serial, tuple(reused), tuple(slots))
+        key = (int(max_new_tokens), tuple(tuple(p) for p in prompts), gkey, cont)
+        p = self._llm_plans.get(key)
+        if p is None:
             L = _lib.lib()
-            flat = [int(t) for p in prompts for t in p]
+            B = len(prompts)
+            flat = [int(t) for q in prompts for t in q]
             ids = (ctypes.c_int32 * len(flat))(*flat)
-            lens = (ctypes.c_int32 * len(prompts))(*[len(p) for p in prompts])
+            lens = (ctypes.c_int32 * B)(*[len(q) for q in prompts])
             garr = (ctypes.c_int32 * max(1, len(gkey)))(*gkey)
+            per_seq = lambda v: None if pool is None else (ctypes.c_int32 * B)(*v)
             p = c_void_p()
             with torch.cuda.device(self.device):
-                check(L.n1_llm_plan_create(self._h(), ids, lens, len(prompts), garr, len(gkey) // 3, ctypes.byref(p),
-                                           _lib.stream_ptr()))
+                check(L.n1_llm_plan_create(self._h(), ids, lens, B, garr, len(gkey) // 3, int(max_new_tokens),
+                                           None if pool is None else pool._p, per_seq(reused), per_seq(slots),
+                                           ctypes.byref(p), _lib.stream_ptr()))
             self._evict_plans(L)
-            hit = (p, len(prompts))
-            self._llm_plans[key] = hit
-        return hit[0]
+            self._llm_plans[key] = p
+        return p
 
     def _evict_plans(self, L, keep=8):
         """Prompts change every step in deployment, so the cache only serves repeated calls within a step (generate +
@@ -444,8 +336,7 @@ class System2:
         finished long ago, so the recycling never has to wait."""
         while len(self._llm_plans) > keep:
             k = next(iter(self._llm_plans))
-            old, _ = self._llm_plans.pop(k)
-            L.n1_llm_plan_destroy(old)
+            L.n1_llm_plan_destroy(self._llm_plans.pop(k))
 
     def positions(self, plan, B):
         L = _lib.lib()
@@ -456,36 +347,29 @@ class System2:
         return torch.tensor(list(pos), dtype=torch.int64).view(3, n), torch.tensor(list(dl), dtype=torch.int64)
 
     # ------------------------------------------------------------------ hot calls
-    def visual(self, pixel_values, grid_thw):
-        """self.visual(pixel_values, grid_thw=image_grid_thw): [N, 1176] -> [N/4, hidden] bf16."""
+    def visual(self, pixel_values, grid_thw, feature_pool=None, dst_rows=None):
+        """self.visual(pixel_values, grid_thw=image_grid_thw): [N, 1176] -> [N/4, hidden] bf16.  With an ImageFeaturePool
+        merged row r goes to feature_pool.feats[dst_rows[r]] instead (int32, no row twice) and nothing is returned."""
         L = _lib.lib()
         plan = self.vit_plan(grid_thw)
         px = pixel_values.to(self.device, torch.bfloat16).contiguous()
         n = L.n1_vit_plan_patches(plan)
         assert px.shape[0] == n, "pixel_values rows (%d) do not match image_grid_thw (%d patches)" % (px.shape[0], n)
-        out = torch.empty(n // (self.cfg["v_merge"] ** 2), self.cfg["v_out"], device=self.device, dtype=torch.bfloat16)
+        if feature_pool is None:
+            out, dst = torch.empty(n // (self.cfg["v_merge"] ** 2), self.cfg["v_out"], device=self.device,
+                                   dtype=torch.bfloat16), None
+        else:
+            out, dst = feature_pool.feats, np.ascontiguousarray(dst_rows, dtype=np.int32)
         nb = L.n1_vit_workspace_bytes(self._h(), plan)
         ws = self._scratch("vit", nb)
-        check(L.n1_qwen_vit(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(out), _lib.stream_ptr()))
-        return out
-
-    def visual_rows(self, pixel_values, grid_thw, feature_pool, dst_rows):
-        """visual() writing merged row r to feature_pool.feats[dst_rows[r]] (int32, no row twice) instead of a new tensor."""
-        L = _lib.lib()
-        plan = self.vit_plan(grid_thw)
-        px = pixel_values.to(self.device, torch.bfloat16).contiguous()
-        n = L.n1_vit_plan_patches(plan)
-        assert px.shape[0] == n, "pixel_values rows (%d) do not match image_grid_thw (%d patches)" % (px.shape[0], n)
-        dst = np.ascontiguousarray(dst_rows, dtype=np.int32)
-        nb = L.n1_vit_workspace_bytes(self._h(), plan)
-        ws = self._scratch("vit", nb)
-        check(L.n1_qwen_vit_rows(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(feature_pool.feats),
-                                 feature_pool.rows, _i32(dst), len(dst), _lib.stream_ptr()))
+        check(L.n1_qwen_vit(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(out), out.shape[0],
+                            None if dst is None else _i32(dst), 0 if dst is None else len(dst), _lib.stream_ptr()))
+        return out if feature_pool is None else None
 
     def _pool_features(self, feature_pool, px, grid_thw, digests, images):
         """Image features of grid_thw[i] for i in `images` (in plan order) through `feature_pool`: the images it does not
         hold go through the vision tower in one call, into freshly taken rows.  -> (int32 row table of the plan's image
-        tokens, patches encoded, images served from the pool).  Sets self.last_features."""
+        tokens, patches encoded).  Sets self.last_features."""
         merge2 = self.cfg["v_merge"] ** 2
         sizes = [int(t) * int(h) * int(w) for t, h, w in grid_thw]
         start = np.concatenate([[0], np.cumsum(sizes)]).tolist()
@@ -500,14 +384,14 @@ class System2:
         if miss:
             try:
                 sub = torch.cat([px[start[i]:start[i + 1]] for i, _ in miss]) if len(miss) < len(grid_thw) else px
-                self.visual_rows(sub, [grid_thw[i] for i, _ in miss], feature_pool, np.concatenate([r for _, r in miss]))
+                self.visual(sub, [grid_thw[i] for i, _ in miss], feature_pool, np.concatenate([r for _, r in miss]))
             except Exception:
                 feature_pool.discard(new)
                 raise
         patches = sum(sizes[i] for i, _ in miss)
         self.last_features = dict(image_hits=hits, vit_patches=patches)
         table = np.concatenate(rows) if rows else np.zeros(0, dtype=np.int32)
-        return table, patches, hits
+        return table, patches
 
     def prefill_latents(self, prompts, image_feats, grid_thw):
         """Embedding splice + decoder prefill + last-n_query slice for B prompts -> [B, n_query, hidden] bf16."""
@@ -531,7 +415,7 @@ class System2:
         """Hidden states at the TRAJ positions for a training batch (prompts WITHOUT the TRAJ tokens): [B, n_query, H].
         Keeps the K/V cache and the per-layer TRAJ-row tensors for `train_backward` (same prompts, next call)."""
         L = _lib.lib()
-        plan = self.gen_plan(prompts, grid_thw, 1)
+        plan = self.llm_plan(prompts, grid_thw, 1)
         feats = self.visual(pixel_values, grid_thw) if image_feats is None else image_feats
         feats = feats.to(self.device, torch.bfloat16).contiguous()
         out = torch.empty(len(prompts), self.cfg["n_query"], self.cfg["hidden"], device=self.device, dtype=torch.bfloat16)
@@ -556,70 +440,94 @@ class System2:
                                               _lib.stream_ptr()))
         return out
 
-    def gen_plan(self, prompts, grid_thw, max_new_tokens):
-        gkey = tuple(int(v) for g in grid_thw for v in g)
-        key = ("gen", int(max_new_tokens), tuple(tuple(p) for p in prompts), gkey)
-        hit = self._llm_plans.get(key)
-        if hit is None:
-            L = _lib.lib()
-            flat = [int(t) for p in prompts for t in p]
-            ids = (ctypes.c_int32 * len(flat))(*flat)
-            lens = (ctypes.c_int32 * len(prompts))(*[len(p) for p in prompts])
-            garr = (ctypes.c_int32 * max(1, len(gkey)))(*gkey)
-            p = c_void_p()
-            with torch.cuda.device(self.device):
-                check(L.n1_gen_plan_create(self._h(), ids, lens, len(prompts), garr, len(gkey) // 3, int(max_new_tokens),
-                                           ctypes.byref(p), _lib.stream_ptr()))
-            self._evict_plans(L)
-            hit = (p, len(prompts))
-            self._llm_plans[key] = hit
-        return hit[0]
-
     def generate(self, prompts, pixel_values, grid_thw, max_new_tokens=128, eos_token_ids=EOS_TOKEN_IDS,
                  pad_token_id=PAD_TOKEN_ID, with_latents=False, image_feats=None, past_key_values=None, feature_pool=None):
         """Greedy decode for B prompts (`model.generate(do_sample=False, max_new_tokens=...)`, internvla_n1_policy.py
         L169-176).  Returns (list of B generated-token lists, each ending with its eos id unless the budget ran out,
         latents [B, n_query, hidden] or None, decode passes run).  With `with_latents` the K/V cache of the decode is
         extended by the TRAJ tokens, which equals `generate_latents(output_ids, ...)` without a second prefill.
-        `past_key_values`: one KVCache per prompt (see _generate_cached); the call then also sets `self.last_cache`.
+        `image_feats`: the vision tower's output for every image, used instead of `pixel_values`.
+        `past_key_values`: one entry per prompt, a KVCache of one KVPool (an empty one for a fresh prompt; all slots
+        distinct) or None: a fresh conversation on a slot no other entry uses (one never written if there is one, else the
+        lowest; a cache held elsewhere on that slot goes stale).  Prompt b reuses reuse_length(...) rows of its slot: only
+        the images after that prefix go through the vision tower and only the rows after it are prefilled.  Afterwards the
+        slot holds the new conversation and `self.last_cache` = dict(caches=[one new KVCache per prompt], prefill_rows,
+        vit_patches, reused).  A batch in which some conversation does not fit its slot runs as an uncached call and
+        returns None for every cache.
         `feature_pool`: an ImageFeaturePool; images it holds skip the vision tower, the others are encoded into it, and
         `self.last_features` = dict(image_hits, vit_patches).  The outputs are byte-identical to a call without it."""
-        if feature_pool is not None and image_feats is not None:
-            raise ValueError("generate: image_feats and feature_pool exclude each other")
+        if image_feats is not None and (feature_pool is not None or past_key_values is not None):
+            raise ValueError("generate: image_feats excludes feature_pool and past_key_values")
+        B, nq = len(prompts), self.cfg["n_query"]
+        caches = pool = None
         if past_key_values is not None:
-            return self._generate_cached(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
-                                         with_latents, past_key_values, feature_pool)
+            if len(past_key_values) != B or all(c is None for c in past_key_values):
+                raise ValueError("past_key_values: one KVCache or None per prompt, at least one KVCache")
+            given = [c for c in past_key_values if c is not None]
+            pool = given[0].pool
+            if any(c.pool is not pool for c in given) or len({c.slot for c in given}) != len(given):
+                raise ValueError("past_key_values: the caches of one call must be distinct slots of one KVPool")
+            # a None entry starts a fresh conversation on a slot no other entry uses: one never written first, then the lowest
+            free = sorted((s_ for s_ in range(pool.slots) if s_ not in {c.slot for c in given}),
+                          key=lambda s_: (pool.valid(s_) > 0, s_))
+            if len(free) < B - len(given):
+                raise ValueError("past_key_values: the pool has no free slot for a None entry")
+            free = iter(free)
+            caches = [c if c is not None else pool.handle(next(free)) for c in past_key_values]
+            if any(len(p) + int(max_new_tokens) + nq > pool.capacity for p in prompts):
+                pool = None   # some conversation does not fit its slot: an uncached call
         L = _lib.lib()
         if not L.n1_s2_has_lm_head(self._h()):
             raise RuntimeError("generate() needs lm_head.weight in the loaded state_dict; there is no fallback")
-        plan = self.gen_plan(prompts, grid_thw, max_new_tokens)
-        B = len(prompts)
-        table = None
+        px = None if image_feats is not None else pixel_values.to(self.device, torch.bfloat16).contiguous()
+        digests = self.image_digests(px, grid_thw) if pool is not None or feature_pool is not None else None
+        # the rows each prompt reuses, and the images after that prefix: only those need features
+        reused, keep, images = [0] * B, list(range(len(grid_thw))), []
+        if pool is not None:
+            keep, gi = [], 0
+            for b, (p, c) in enumerate(zip(prompts, caches)):
+                spans = image_spans(p, grid_thw[gi:], self.cfg["v_merge"])
+                imgs = [(st, n, digests[gi + k]) for k, (st, n) in enumerate(spans)]
+                r = reuse_length(c.tokens, c.images, p, imgs, pool.capacity, len(p) + int(max_new_tokens) + nq) \
+                    if len(c) else 0
+                reused[b] = min(r, pool.valid(c.slot)) if r else 0
+                keep += [gi + k for k, (st, _, _) in enumerate(imgs) if st >= reused[b]]
+                images.append({st: (n, dg) for st, n, dg in imgs})
+                gi += len(spans)
+        sizes = [int(t) * int(h) * int(w) for t, h, w in grid_thw]
+        feats, table = image_feats, None
         if feature_pool is not None:
-            px = pixel_values.to(self.device, torch.bfloat16).contiguous()
-            table, _, _ = self._pool_features(feature_pool, px, grid_thw, self.image_digests(px, grid_thw),
-                                              range(len(grid_thw)))
+            table, vit_patches = self._pool_features(feature_pool, px, grid_thw, digests, keep)
             feats = feature_pool.feats
         else:
-            feats = self.visual(pixel_values, grid_thw) if image_feats is None else image_feats
+            vit_patches = sum(sizes[i] for i in keep)
+            if feats is None and keep:
+                start = np.cumsum([0] + sizes).tolist()
+                sub = px if len(keep) == len(grid_thw) else torch.cat([px[start[i]:start[i + 1]] for i in keep])
+                feats = self.visual(sub, [grid_thw[i] for i in keep])
+        if feats is not None:
             feats = feats.to(self.device, torch.bfloat16).contiguous()
-            assert feats.shape[0] == L.n1_llm_plan_image_tokens(plan), "image features and image tokens do not match"
-        lat = torch.empty(B, self.cfg["n_query"], self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) \
-            if with_latents else None
-        nb = L.n1_generate_workspace_bytes(self._h(), plan)
+        slots = None if pool is None else [c.slot for c in caches]
+        plan = self.llm_plan(prompts, grid_thw, max_new_tokens, pool, reused, slots)
+        lat = torch.empty(B, nq, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) if with_latents else None
+        nb = L.n1_llm_workspace_bytes(self._h(), plan)
         ws = self._scratch("gen", nb)
         eos = (ctypes.c_int32 * max(1, len(eos_token_ids)))(*[int(e) for e in eos_token_ids])
         toks = (ctypes.c_int32 * (B * int(max_new_tokens)))()
         lens = (ctypes.c_int32 * B)()
         passes = ctypes.c_int32(0)
-        if table is None:
-            check(L.n1_llm_generate(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), eos, len(eos_token_ids),
-                                    int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
-        else:
-            check(L.n1_llm_generate_rows(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), feature_pool.rows, _i32(table),
-                                         len(table), eos, len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
-                                         ctypes.byref(passes), _lib.stream_ptr()))
+        for s_ in slots or ():   # the call rewrites these slots: every older handle on them is stale from here on
+            pool.version[s_] += 1
+        check(L.n1_llm_generate(self._h(), plan, _lib.ptr(ws), nb, _lib.ptr(feats), 0 if feats is None else feats.shape[0],
+                                None if table is None else _i32(table), 0 if table is None else len(table), eos,
+                                len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes),
+                                _lib.stream_ptr()))
         out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
+        if caches is not None:
+            new = [None] * B if pool is None else \
+                [KVCache(pool, s_, (p + o)[:pool.valid(s_)], im) for p, o, s_, im in zip(prompts, out, slots, images)]
+            self.last_cache = dict(caches=new, prefill_rows=int(L.n1_llm_plan_tokens(plan)), vit_patches=vit_patches,
+                                   reused=reused)
         return out, lat, passes.value
 
     def image_digests(self, px, grid_thw):
@@ -630,117 +538,3 @@ class System2:
         check(_lib.lib().n1_image_digest(_lib.ptr(px), px.shape[1], _lib.ptr(off), len(sizes), _lib.ptr(out),
                                          _lib.stream_ptr()))
         return out.tolist()
-
-    def _generate_cached(self, prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id, with_latents,
-                         caches, feature_pool=None):
-        """generate() continuing cached conversations.  caches[b] is a KVCache of one KVPool (an empty one for a fresh
-        prompt; all slots distinct) or None: a fresh conversation on a slot no other entry uses (one never written if
-        there is one, else the lowest; a cache held elsewhere on that slot goes stale).  Prompt b reuses reuse_length(...) rows of its slot: only the images after that
-        prefix go through the vision tower and only the rows after it are prefilled.  Afterwards the slot holds the new
-        conversation and `self.last_cache` = dict(caches=[one new KVCache per prompt], prefill_rows, vit_patches, reused).
-        A batch in which some conversation does not fit its slot runs as an uncached call and returns no caches."""
-        L = _lib.lib()
-        B = len(prompts)
-        if len(caches) != B or all(c is None for c in caches):
-            raise ValueError("past_key_values: one KVCache or None per prompt, at least one KVCache")
-        pool = next(c for c in caches if c is not None).pool
-        given = [c for c in caches if c is not None]
-        if any(c.pool is not pool for c in given) or len({c.slot for c in given}) != len(given):
-            raise ValueError("past_key_values: the caches of one call must be distinct slots of one KVPool")
-        # a None entry starts a fresh conversation on a slot no other entry uses: one never written first, then the lowest
-        free = sorted((s_ for s_ in range(pool.slots) if s_ not in {c.slot for c in given}),
-                      key=lambda s_: (pool.valid(s_) > 0, s_))
-        if len(free) < B - len(given):
-            raise ValueError("past_key_values: the pool has no free slot for a None entry")
-        free = iter(free)
-        caches = [c if c is not None else pool.handle(next(free)) for c in caches]
-        nq, merge = self.cfg["n_query"], self.cfg["v_merge"]
-        need = [len(p) + int(max_new_tokens) + nq for p in prompts]
-        if any(n > pool.capacity for n in need):
-            toks, lat, passes = self.generate(prompts, pixel_values, grid_thw, max_new_tokens, eos_token_ids, pad_token_id,
-                                              with_latents, feature_pool=feature_pool)
-            n_p = sum(int(t) * int(h) * int(w) for t, h, w in grid_thw) if feature_pool is None else \
-                self.last_features["vit_patches"]
-            self.last_cache = dict(caches=[None] * B, prefill_rows=sum(len(p) for p in prompts), vit_patches=n_p,
-                                   reused=[0] * B)
-            return toks, lat, passes
-        px = pixel_values.to(self.device, torch.bfloat16).contiguous()
-        digests = self.image_digests(px, grid_thw)
-        reused, keep_rows, keep_grids, keep_idx, images = [], [], [], [], []
-        gi, row = 0, 0
-        for b, (p, c) in enumerate(zip(prompts, caches)):
-            spans = image_spans(p, grid_thw[gi:], merge)
-            imgs = [(st, n, digests[gi + k]) for k, (st, n) in enumerate(spans)]
-            r = reuse_length(c.tokens, c.images, p, imgs, pool.capacity, need[b]) if len(c) else 0
-            r = min(r, pool.valid(c.slot)) if r else 0
-            for k, (st, n, dg) in enumerate(imgs):  # patch rows of the images after the reused prefix
-                t, h, w = (int(v) for v in grid_thw[gi + k])
-                if st >= r:
-                    keep_rows.append((row, row + t * h * w))
-                    keep_grids.append(grid_thw[gi + k])
-                    keep_idx.append(gi + k)
-                row += t * h * w
-            reused.append(r)
-            images.append({st: (n, dg) for st, n, dg in imgs})
-            gi += len(spans)
-        table = None
-        if feature_pool is not None:
-            table, vit_patches, _ = self._pool_features(feature_pool, px, grid_thw, digests, keep_idx)
-            feats = feature_pool.feats
-        elif keep_rows:
-            sub = px if len(keep_rows) == len(grid_thw) else torch.cat([px[a:e] for a, e in keep_rows])
-            feats = self.visual(sub, keep_grids)
-        else:
-            feats = torch.empty(0, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16)
-        if feature_pool is None:
-            vit_patches = sum(e - a for a, e in keep_rows)
-        slots = [c.slot for c in caches]
-        plan = self._cont_plan(prompts, grid_thw, max_new_tokens, pool, reused, slots)
-        assert table is not None or feats.shape[0] == L.n1_llm_plan_image_tokens(plan), \
-            "image features and image tokens do not match"
-        lat = torch.empty(B, nq, self.cfg["hidden"], device=self.device, dtype=torch.bfloat16) if with_latents else None
-        nb = L.n1_generate_workspace_bytes(self._h(), plan)
-        ws = self._scratch("gen", nb)
-        eos = (ctypes.c_int32 * max(1, len(eos_token_ids)))(*[int(e) for e in eos_token_ids])
-        toks = (ctypes.c_int32 * (B * int(max_new_tokens)))()
-        lens = (ctypes.c_int32 * B)()
-        passes = ctypes.c_int32(0)
-        for s_ in slots:  # the call rewrites these slots: every older handle on them is stale from here on
-            pool.version[s_] += 1
-        if table is None:
-            check(L.n1_llm_generate_pool(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), eos,
-                                         len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat),
-                                         ctypes.byref(passes), _lib.stream_ptr()))
-        else:
-            check(L.n1_llm_generate_pool_rows(self._h(), plan, pool._p, _lib.ptr(ws), nb, _lib.ptr(feats), feature_pool.rows,
-                                              _i32(table), len(table), eos, len(eos_token_ids), int(pad_token_id), toks,
-                                              lens, _lib.ptr(lat), ctypes.byref(passes), _lib.stream_ptr()))
-        out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
-        new = []
-        for b, p in enumerate(prompts):
-            valid = pool.valid(slots[b])
-            new.append(KVCache(pool, slots[b], (p + out[b])[:valid], images[b]))
-        self.last_cache = dict(caches=new, prefill_rows=int(L.n1_llm_plan_tokens(plan)),
-                               vit_patches=vit_patches, reused=reused)
-        return out, lat, passes.value
-
-    def _cont_plan(self, prompts, grid_thw, max_new_tokens, pool, reused, slots):
-        gkey = tuple(int(v) for g in grid_thw for v in g)
-        key = ("cont", pool.serial, int(max_new_tokens), tuple(tuple(p) for p in prompts), gkey, tuple(reused), tuple(slots))
-        hit = self._llm_plans.get(key)
-        if hit is None:
-            L = _lib.lib()
-            flat = [int(t) for p in prompts for t in p]
-            ids = (ctypes.c_int32 * len(flat))(*flat)
-            lens = (ctypes.c_int32 * len(prompts))(*[len(p) for p in prompts])
-            garr = (ctypes.c_int32 * max(1, len(gkey)))(*gkey)
-            ctx = (ctypes.c_int32 * len(prompts))(*reused)
-            sl = (ctypes.c_int32 * len(prompts))(*slots)
-            p = c_void_p()
-            with torch.cuda.device(self.device):
-                check(L.n1_gen_plan_create_cont(self._h(), ids, lens, len(prompts), garr, len(gkey) // 3,
-                                                int(max_new_tokens), pool._p, ctx, sl, ctypes.byref(p), _lib.stream_ptr()))
-            self._evict_plans(L)
-            hit = (p, len(prompts))
-            self._llm_plans[key] = hit
-        return hit[0]

@@ -1,6 +1,7 @@
 """Decode-pass timing of n1_llm_generate at the dual-system bench shape (Qwen2.5-VL-7B, random weights, B prompts of
-S = 300 tokens incl. one 392x392 image): wall time of generate(max_new = a) vs generate(max_new = b) -> ms per decode
-pass, against the weight-streaming floor (all decoder + lm_head weights once per pass at the measured HBM bandwidth)."""
+S = 300 tokens incl. one 392x392 image), on a generation plan without a K/V pool and with the image features passed
+whole (no row table): wall time of generate(max_new = a) vs generate(max_new = b) -> ms per decode pass, against the
+weight-streaming floor (all decoder + lm_head weights once per pass at the measured HBM bandwidth)."""
 import argparse
 import json
 import os

@@ -77,25 +77,20 @@ def test_null_arguments_are_errors():
     L.n1_destroy(None)  # no-op
 
 
-def test_ctypes_signatures_have_the_declared_arity():
-    """Every ctypes binding in the package passes as many arguments as include/n1b200.h declares (a mismatch would
-    corrupt the call silently)."""
+def test_every_declared_symbol_is_bound_with_its_arity():
+    """Every function include/n1b200.h declares has a ctypes binding that passes as many arguments as the header declares
+    (a mismatch would corrupt the call silently)."""
     import re
-    from internnav_b200 import _bwd, _lib, preprocess, qwen
+    from internnav_b200 import _lib
     L = _lib.lib()
-    qwen._bind(L)
-    preprocess._bind(L)
-    _bwd._L()
     with open(os.path.join(ROOT, "include", "n1b200.h")) as fh:
         src = re.sub(r"/\*.*?\*/", "", fh.read(), flags=re.S)
     decl = {}
     for m in re.finditer(r"\b(n1_[a-z0-9_]+)\s*\(([^;{]*?)\)\s*;", src, flags=re.S):
         args = m.group(2).strip()
         decl[m.group(1)] = 0 if args in ("", "void") else args.count(",") + 1
-    checked = 0
+    assert len(decl) >= 80 and set(decl) == set(_lib.SYMBOLS), set(decl) ^ set(_lib.SYMBOLS)
     for name, n in decl.items():
         fn = getattr(L, name)
-        if fn.argtypes is not None:
-            assert len(fn.argtypes) == n, "%s: header declares %d arguments, binding passes %d" % (name, n, len(fn.argtypes))
-            checked += 1
-    assert checked >= 45, checked
+        assert fn.argtypes is not None, "%s has no binding" % name
+        assert len(fn.argtypes) == n, "%s: header declares %d arguments, binding passes %d" % (name, n, len(fn.argtypes))

@@ -73,14 +73,13 @@ def test_training_prefix_extraction():
         m.forward(input_ids=ids)                                         # inference-style call: use generate*()
 
 
-def test_resize_plan_needs_a_device():
+def test_resize_plan_create_needs_a_device():
     """Compute entry points fail loudly without an H100 (no host fallback behind the C ABI)."""
     from internnav_b200 import _lib
-    from internnav_b200.preprocess import FramePreprocessor, _bind
+    from internnav_b200.preprocess import FramePreprocessor
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     L = _lib.lib()
-    _bind(L)
     p = ctypes.c_void_p()
     assert L.n1_resize_plan_create(480, 640, 224, 224, ctypes.byref(p), None) != 0
     assert len(L.n1_last_error()) > 0

@@ -172,7 +172,7 @@ def test_mixed_batch_and_uncached_calls():
         assert toks[b] == alone[0], (b, toks[b], alone[0])
 
 
-def test_pool_errors():
+def test_kv_pool_plan_and_generate_errors():
     from internnav_b200 import _lib
     from internnav_b200.qwen import KVPool
     from oracle import qwen_oracle as Q
@@ -189,17 +189,16 @@ def test_pool_errors():
     p = ctypes.c_void_p()
     for reuse, slot, msg in [(0, 5, b"out of range"), (8, 0, b"reused length"), (0, 0, b"capacity")]:
         new = 60 if msg == b"capacity" else 4
-        rc = L.n1_gen_plan_create_cont(s2._h(), ids, lens, 1, (ctypes.c_int32 * 1)(0), 0, new, pool._p,
-                                       (ctypes.c_int32 * 1)(reuse), (ctypes.c_int32 * 1)(slot), ctypes.byref(p),
-                                       _lib.stream_ptr())
+        rc = L.n1_llm_plan_create(s2._h(), ids, lens, 1, (ctypes.c_int32 * 1)(0), 0, new, pool._p,
+                                  (ctypes.c_int32 * 1)(reuse), (ctypes.c_int32 * 1)(slot), ctypes.byref(p), _lib.stream_ptr())
         assert rc == -2 and msg in L.n1_last_error(), L.n1_last_error()
     # a reused length beyond what the slot holds is refused at the call
-    rc = L.n1_gen_plan_create_cont(s2._h(), ids, lens, 1, (ctypes.c_int32 * 1)(0), 0, 4, pool._p, (ctypes.c_int32 * 1)(3),
-                                   (ctypes.c_int32 * 1)(0), ctypes.byref(p), _lib.stream_ptr())
+    rc = L.n1_llm_plan_create(s2._h(), ids, lens, 1, (ctypes.c_int32 * 1)(0), 0, 4, pool._p, (ctypes.c_int32 * 1)(3),
+                              (ctypes.c_int32 * 1)(0), ctypes.byref(p), _lib.stream_ptr())
     assert rc == 0
-    ws = torch.empty(L.n1_generate_workspace_bytes(s2._h(), p), dtype=torch.uint8, device="cuda")
+    ws = torch.empty(L.n1_llm_workspace_bytes(s2._h(), p), dtype=torch.uint8, device="cuda")
     toks, ln = (ctypes.c_int32 * 4)(), (ctypes.c_int32 * 1)()
-    rc = L.n1_llm_generate_pool(s2._h(), p, pool._p, _lib.ptr(ws), ws.numel(), None, None, 0, 0, toks, ln, None, None,
-                                _lib.stream_ptr())
+    rc = L.n1_llm_generate(s2._h(), p, _lib.ptr(ws), ws.numel(), None, 0, None, 0, None, 0, 0, toks, ln, None, None,
+                           _lib.stream_ptr())
     assert rc == -2 and b"holds 0" in L.n1_last_error(), L.n1_last_error()
     L.n1_llm_plan_destroy(p)

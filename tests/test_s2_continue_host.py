@@ -84,9 +84,8 @@ def test_mrope_positions_continue():
 
 
 def _plan_rows(prompts, grids, max_new, reused=None, slots=None, pool=(0, 0), n_query=4):
-    from internnav_b200 import _lib, qwen
+    from internnav_b200 import _lib
     L = _lib.lib()
-    qwen._bind(L)
     i32 = ctypes.c_int32
     flat = [t for p in prompts for t in p]
     g = [v for gr in grids for v in gr]
@@ -102,7 +101,7 @@ def _plan_rows(prompts, grids, max_new, reused=None, slots=None, pool=(0, 0), n_
     return list(cu), list(kind)[:r], list(src)[:r], list(dest)[:r], list(kl)
 
 
-def test_plan_bookkeeping_mixed_batch():
+def test_plan_rows_mixed_batch():
     """A batch of a fresh and a continued sequence: only the continued one's suffix is planned, image features are
     numbered over the suffix images alone, K/V rows land in each sequence's pool slot, and the keys cover the whole prompt."""
     rng = np.random.Generator(np.random.PCG64(2))

@@ -24,7 +24,7 @@ def _px(grids, seed):
     return torch.randn(sum(t * h * w for t, h, w in grids), 1176, generator=g).bfloat16().cuda()
 
 
-def test_features_are_batch_invariant():
+def test_vision_features_are_batch_invariant():
     """Mixed sizes at the 7B vision widths: each image's features alone, in batches of other orders and compositions,
     in a 64-image batch, and written through a row map into a pool are the same bytes."""
     from internnav_b200.qwen import ImageFeaturePool, System2
@@ -55,7 +55,7 @@ def test_features_are_batch_invariant():
     pool.feats.fill_(7.0)
     order = [4, 0, 2]
     dst = np.random.default_rng(0).permutation(4096)[:sum(merged[i] for i in order)].astype(np.int32)
-    s2.visual_rows(torch.cat([pxs[i] for i in order]), [grids[i] for i in order], pool, dst)
+    s2.visual(torch.cat([pxs[i] for i in order]), [grids[i] for i in order], pool, dst)
     got = _bits(pool.feats)
     r = 0
     for i in order:
@@ -151,8 +151,9 @@ def test_small_pool_evicts_and_outputs_stay_identical():
         _run(model, 6, False, model.make_feature_pool(40))
 
 
-def test_row_table_checks():
-    """The entry points refuse a row table of the wrong length or with a row outside the pool, before anything runs."""
+def test_row_table_and_feature_count_checks():
+    """The entry points refuse a row table of the wrong length or with a row outside the pool, and without a row table
+    features of the wrong length, before anything runs."""
     import ctypes
     from internnav_b200 import _lib
     from internnav_b200.qwen import ImageFeaturePool, _i32
@@ -168,8 +169,8 @@ def test_row_table_checks():
 
     def vit(rows):
         a = np.asarray(rows, dtype=np.int32)
-        return L.n1_qwen_vit_rows(s2._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(pool.feats), pool.rows, _i32(a),
-                                  len(a), _lib.stream_ptr()), L.n1_last_error().decode()
+        return L.n1_qwen_vit(s2._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(pool.feats), pool.rows, _i32(a),
+                             len(a), _lib.stream_ptr()), L.n1_last_error().decode()
 
     assert vit(range(16))[0] == 0
     assert vit(range(15))[0] == -2 and "16" in vit(range(15))[1]
@@ -177,17 +178,23 @@ def test_row_table_checks():
     assert rc == -2 and "outside the pool" in msg
     rc, msg = vit([0] * 16)
     assert rc == -2 and "twice" in msg
+    rc = L.n1_qwen_vit(s2._h(), plan, _lib.ptr(ws), nb, _lib.ptr(px), _lib.ptr(pool.feats), pool.rows, None, 0,
+                       _lib.stream_ptr())   # without a table the output has exactly the 16 merged rows
+    assert rc == -2 and "16" in L.n1_last_error().decode(), L.n1_last_error()
     from oracle import qwen_oracle as Q
     prompt = Q.make_prompt(np.random.Generator(np.random.PCG64(1)), 3, grids, 2)
-    gp = s2.gen_plan([prompt], grids, 2)
-    gnb = L.n1_generate_workspace_bytes(s2._h(), gp)
+    gp = s2.llm_plan([prompt], grids, 2)
+    gnb = L.n1_llm_workspace_bytes(s2._h(), gp)
     gws = torch.empty(gnb, dtype=torch.uint8, device="cuda")
     toks, lens = (ctypes.c_int32 * 2)(), (ctypes.c_int32 * 1)()
     for rows, msg in [(range(15), "entries"), (list(range(15)) + [-1], "outside the pool")]:
         a = np.asarray(rows, dtype=np.int32)
-        rc = L.n1_llm_generate_rows(s2._h(), gp, _lib.ptr(gws), gnb, _lib.ptr(pool.feats), pool.rows, _i32(a), len(a), None,
-                                    0, 0, toks, lens, None, None, _lib.stream_ptr())
+        rc = L.n1_llm_generate(s2._h(), gp, _lib.ptr(gws), gnb, _lib.ptr(pool.feats), pool.rows, _i32(a), len(a), None, 0,
+                               0, toks, lens, None, None, _lib.stream_ptr())
         assert rc == -2 and msg in L.n1_last_error().decode(), L.n1_last_error()
+    rc = L.n1_llm_generate(s2._h(), gp, _lib.ptr(gws), gnb, _lib.ptr(pool.feats), 15, None, 0, None, 0, 0, toks, lens, None,
+                           None, _lib.stream_ptr())   # without a table the features have exactly the 16 image-token rows
+    assert rc == -2 and "16" in L.n1_last_error().decode(), L.n1_last_error()
 
 
 def _raw(shape, seed):

@@ -101,25 +101,22 @@ def test_history_hits_match_a_set_count(gap):
     assert share > {2: 0.8, 4: 0.65, 8: 0.45}[gap]
 
 
-def test_row_entry_points_refuse_bad_arguments():
-    """The checks that need no device: a null handle, plan or pool is refused before anything runs."""
-    from internnav_b200 import _lib, qwen
+def test_vit_and_generate_refuse_bad_arguments():
+    """The checks that need no device: a null handle, plan or pixels, or too many eos ids, is refused before anything
+    runs."""
+    from internnav_b200 import _lib
     L = _lib.lib()
-    qwen._bind(L)
     fake = ctypes.c_void_p(1 << 20)
     rows = (ctypes.c_int32 * 4)(0, 1, 2, 3)
     toks, lens = (ctypes.c_int32 * 4)(), (ctypes.c_int32 * 1)()
-    assert L.n1_qwen_vit_rows(None, fake, fake, 1, fake, fake, 8, rows, 4, None) == -2
+    assert L.n1_qwen_vit(None, fake, fake, 1, fake, fake, 8, rows, 4, None) == -2
     assert b"null handle" in L.n1_last_error()
-    assert L.n1_qwen_vit_rows(fake, None, fake, 1, fake, fake, 8, rows, 4, None) == -2
-    assert L.n1_qwen_vit_rows(fake, fake, fake, 1, None, fake, 8, rows, 4, None) == -2
-    assert L.n1_llm_generate_rows(None, fake, fake, 1, fake, 8, rows, 4, None, 0, 0, toks, lens, None, None, None) == -2
-    assert L.n1_llm_generate_rows(fake, None, fake, 1, fake, 8, rows, 4, None, 0, 0, toks, lens, None, None, None) == -2
-    assert L.n1_llm_generate_pool_rows(fake, fake, None, fake, 1, fake, 8, rows, 4, None, 0, 0, toks, lens, None, None,
-                                       None) == -2
-    assert b"null handle / plan / pool" in L.n1_last_error()
-    assert L.n1_llm_generate_pool_rows(fake, fake, fake, fake, 1, fake, 8, rows, 4, None, 5, 0, toks, lens, None, None,
-                                       None) == -2
+    assert L.n1_qwen_vit(fake, None, fake, 1, fake, fake, 8, rows, 4, None) == -2
+    assert L.n1_qwen_vit(fake, fake, fake, 1, None, fake, 8, rows, 4, None) == -2
+    assert L.n1_llm_generate(None, fake, fake, 1, fake, 8, rows, 4, None, 0, 0, toks, lens, None, None, None) == -2
+    assert L.n1_llm_generate(fake, None, fake, 1, fake, 8, rows, 4, None, 0, 0, toks, lens, None, None, None) == -2
+    assert b"null handle / plan" in L.n1_last_error()
+    assert L.n1_llm_generate(fake, fake, fake, 1, fake, 8, rows, 4, None, 5, 0, toks, lens, None, None, None) == -2
     assert b"eos" in L.n1_last_error()
 
 

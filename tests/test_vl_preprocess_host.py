@@ -102,17 +102,16 @@ def test_qualification_rule():
         assert QwenImagePreprocessor.from_hf(ip, "cuda:0") is None, ip
 
 
-def test_patchify_argument_errors():
+def test_vl_patchify_argument_errors():
     """Every argument check runs before the device is touched, so the codes are the same with and without a GPU."""
-    from internnav_b200 import _lib, preprocess
+    from internnav_b200 import _lib
     L = _lib.lib()
-    preprocess._bind(L)
     fake = ctypes.c_void_p(1 << 20)
     ws = L.n1_vl_patchify_workspace_bytes(2)
-    assert ws >= 2 * ctypes.sizeof(preprocess.VlImage) and ctypes.sizeof(preprocess.VlImage) == 24
+    assert ws >= 2 * ctypes.sizeof(_lib.VlImage) and ctypes.sizeof(_lib.VlImage) == 24
 
     def call(table, n_rows, ws_bytes=ws, lut=fake, out=fake):
-        arr = (preprocess.VlImage * len(table))(*[preprocess.VlImage(*t) for t in table])
+        arr = (_lib.VlImage * len(table))(*[_lib.VlImage(*t) for t in table])
         return L.n1_vl_patchify(arr, len(table), lut, out, n_rows, fake, ws_bytes, None), L.n1_last_error().decode()
 
     good = [(1 << 20, 392, 392, 0), (1 << 21, 476, 644, 784)]
