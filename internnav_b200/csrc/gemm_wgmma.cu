@@ -10,7 +10,8 @@
 // for 168 registers per thread; after the barrier set-up the producer warpgroup shrinks to 40 and the consumers grow to
 // 232 (setmaxnreg), which holds the 128 accumulators of the 256-wide tile plus the epilogue without spilling.
 //
-// This one kernel carries every Linear / Conv-as-GEMM on the InternVLA-N1 hot path (SURVEY.md §2.1):
+// This kernel, one instance per tile width and epilogue kind, carries every Linear / Conv-as-GEMM on the InternVLA-N1 hot
+// path (SURVEY.md §2.1):
 // the reference reaches cuBLAS through nn.Linear at navdp.py L57-66/L94-100, navdp_backbone.py L147-149,
 // dinov2_layers/{attention.py L46-48, mlp.py L30-32, patch_embed.py L65} and the Qwen2.5-VL blocks.
 #include <stdlib.h>
@@ -40,7 +41,7 @@ struct Cfg {
   static constexpr int kStages = BN == 256 ? 4 : BN == 128 ? 6 : 8;
   static constexpr int kBarBytes = 256;
   static constexpr int kStoreBytes = kConsumerWarps * 2 * 1024;  // per-warp double-buffered 16x32 bf16 staging for TMA stores
-  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + kStoreBytes + 1024;  // +1024: manual alignment
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStoreBytes + kBarBytes + 1024;  // +1024: manual alignment
 };
 static_assert(Cfg<256>::kSmemBytes <= 232448 && Cfg<128>::kSmemBytes <= 232448 && Cfg<64>::kSmemBytes <= 232448,
               "GEMM shared memory budget (227 KB per block)");
@@ -60,8 +61,7 @@ struct GemmArgs {
   int out_fp32;
   int rows_per_group, group_stride, group_offset;
   const float* row_add;
-  int raster_g;   // M tiles per raster group (decode_tile)
-  int tma_store;  // bf16 output tile goes registers -> smem staging -> cp.async.bulk.tensor store (full-sector writes)
+  int raster_g;  // M tiles per raster group (decode_tile)
 };
 
 // Grouped rasterisation: consecutive tile ids walk G M-tiles before moving to the next N-tile, so the CTAs resident at
@@ -77,28 +77,159 @@ __device__ __forceinline__ void decode_tile(int tile, int tiles_m, int tiles_n, 
   tn = r / gsize;
 }
 
-__device__ __forceinline__ float apply_act(float v, int act) {
-  if (act == ACT_GELU) return gelu_erf(v);
-  if (act == ACT_RELU) return fmaxf(v, 0.0f);
-  if (act == ACT_GELU_TANH)  // nn.GELU(approximate="tanh"): the NextDiT condition projections
+// Epilogue kinds.  Each kind is its own compile-time instance of the epilogue below, so an unrolled accumulator loop only
+// carries the code of the kind it runs: a tile's epilogue walks a few KB of machine code instead of every activation,
+// store path and option inlined at each of its BN / 2 accumulator positions.
+//   KIND_LINEAR_SWIGLU  gemm_kernel<BN>: bf16 TMA-store output, acc + bias, then either layer-scale + residual (act none:
+//                       every System-2 GEMM but gate/up and the merger's first layer) or SwiGLU (gate/up), picked once
+//                       per tile
+//   ACT_GELU, ACT_RELU, ACT_GELU_TANH, ACT_SILU   gemm_act_kernel<BN, act>: the same bf16 TMA-store output with one
+//                       activation
+//   KIND_GENERAL        gemm_act_kernel<BN, KIND_GENERAL>: fp32 output, the output row remap, row_add and outputs no
+//                       tensor map can describe, with direct stores; the activation is picked once per tile
+constexpr int KIND_LINEAR_SWIGLU = ACT_NONE;
+constexpr int KIND_GENERAL = 8;
+
+template <int ACT>
+__device__ __forceinline__ float apply_act(float v) {
+  if constexpr (ACT == ACT_GELU) return gelu_erf(v);
+  else if constexpr (ACT == ACT_RELU) return fmaxf(v, 0.0f);
+  else if constexpr (ACT == ACT_GELU_TANH)  // nn.GELU(approximate="tanh"): the NextDiT condition projections
     return 0.5f * v * (1.0f + tanhf(0.7978845608028654f * (v + 0.044715f * v * v * v)));
-  if (act == ACT_SILU) return silu(v);
-  return v;
+  else if constexpr (ACT == ACT_SILU) return silu(v);
+  else return v;
 }
 
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const GemmArgs args) {
+// Epilogue of one tile from the accumulator fragments, for one activation ACT and one store path.  Per element:
+// acc + bias -> activation -> layer-scale -> row_add -> residual -> bf16 / fp32 (SwiGLU: (acc + bias) of a (gate, up)
+// column pair -> silu(gate) * up).  TMA: the bf16 tile leaves through the warp's staging buffer and bulk tensor stores;
+// otherwise direct stores (fp32, the row remap, row_add).
+template <int BN, int ACT, bool TMA>
+__device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], const GemmArgs& args, const CUtensorMap* tmC, int tm,
+                                         int tn, int wrow, int lane, uint8_t* my_store, int& sbuf) {
+  constexpr bool kSwiglu = ACT == ACT_SWIGLU;
+  const int quad = lane & 3;
+  // this thread holds rows r[0], r[1] = r[0] + 8 and, per 8-column group, 2 adjacent columns
+  int row[2];
+  long out_row[2];
+  int grp_row[2] = {0, 0};
+  bool row_ok[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    row[h] = tm * BM + wrow + (lane >> 2) + h * 8;
+    row_ok[h] = row[h] < args.M;
+    out_row[h] = row[h];
+    if (!TMA && args.rows_per_group > 0) {
+      grp_row[h] = row[h] % args.rows_per_group;
+      out_row[h] = (long)(row[h] / args.rows_per_group) * args.group_stride + grp_row[h] + args.group_offset;
+    }
+  }
+#pragma unroll
+  for (int chunk = 0; chunk < BN / 32; ++chunk) {  // unrolled: the accumulator is indexed statically
+    const int col0 = tn * BN + chunk * 32;
+    if (col0 >= args.N) break;  // block-uniform
+    float v[4][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int col = col0 + j * 8 + quad * 2;
+      const bool col_ok = col < args.N;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[j][e] = acc[(chunk * 4 + j) * 4 + e];
+      if (args.bias && col_ok) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(args.bias + col));
+        v[j][0] += b.x, v[j][1] += b.y, v[j][2] += b.x, v[j][3] += b.y;
+      }
+      if constexpr (kSwiglu) {  // (gate, up) interleaved: this thread's column pair -> one output
+        v[j][0] = silu(v[j][0]) * v[j][1];
+        v[j][2] = silu(v[j][2]) * v[j][3];
+      } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[j][e] = apply_act<ACT>(v[j][e]);
+        if (args.gamma && col_ok) {
+          const float2 g = __ldg(reinterpret_cast<const float2*>(args.gamma + col));
+          v[j][0] *= g.x, v[j][1] *= g.y, v[j][2] *= g.x, v[j][3] *= g.y;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h] || !col_ok) continue;
+          if (!TMA && args.row_add) {
+            const float2 a = __ldg(reinterpret_cast<const float2*>(args.row_add + (long)grp_row[h] * args.N + col));
+            v[j][2 * h] += a.x, v[j][2 * h + 1] += a.y;
+          }
+          if (args.residual) {
+            const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(args.residual + out_row[h] * args.ldr + col));
+            v[j][2 * h] += bf16_lo(q), v[j][2 * h + 1] += bf16_hi(q);
+          }
+        }
+      }
+    }
+    if constexpr (TMA) {
+      // 16 rows x 32 columns (SwiGLU: 16 output columns) staged per warp, then one bulk tensor store.  The staging
+      // buffer is 1024-byte aligned and in the tensor map's swizzled layout, which XORs the 16-byte chunk index of a
+      // row with the row's address bits 7 and up: 64-byte rows (SWIZZLE_64B) chunk ^= (r >> 1) & 3, 32-byte rows
+      // (SWIZZLE_32B) chunk ^= (r >> 2) & 1.  One warp's store then hits every bank once: 4-byte words
+      // 16 r + 4 (j ^ (r >> 1) & 3) + quad over r = 0..7, quad = 0..3 are 32 distinct banks (unswizzled: 4-way
+      // conflict); SwiGLU's 2-byte stores, 8 r + 4 ((j >> 1) ^ (r >> 2) & 1) + 2 (j & 1) + quad / 2, are 16 distinct
+      // banks with two lanes per word (unswizzled: 2-way).
+      if (lane == 0) tma_store_wait_read<1>();
+      __syncwarp();
+      uint8_t* sb = my_store + sbuf * 1024;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = (lane >> 2) + h * 8;
+          if constexpr (kSwiglu)
+            *reinterpret_cast<bf16*>(sb + r * 32 + ((((j >> 1) ^ (r >> 2)) & 1) << 4) + (j & 1) * 8 + quad * 2) =
+                __float2bfloat16_rn(v[j][2 * h]);
+          else
+            *reinterpret_cast<uint32_t*>(sb + r * 64 + (((j ^ (r >> 1)) & 3) << 4) + quad * 4) =
+                pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
+        }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) {
+        // rows >= M / cols >= N are clipped by the tensor map
+        tma_store_2d(tmC, sb, kSwiglu ? col0 >> 1 : col0, tm * BM + wrow);
+        tma_store_commit();
+      }
+      sbuf ^= 1;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int col = col0 + j * 8 + quad * 2;
+        if (col >= args.N) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!row_ok[h]) continue;
+          if constexpr (kSwiglu)
+            reinterpret_cast<bf16*>(args.out)[out_row[h] * args.ldo + (col >> 1)] = __float2bfloat16_rn(v[j][2 * h]);
+          else if (args.out_fp32)
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(args.out) + out_row[h] * args.ldo + col) =
+                make_float2(v[j][2 * h], v[j][2 * h + 1]);
+          else
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(args.out) + out_row[h] * args.ldo + col) =
+                pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
+        }
+      }
+    }
+  }
+}
+
+// The persistent kernel with the epilogue of KIND (above); every kind but KIND_GENERAL stores through TMA.
+template <int BN, int KIND>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                                          const GemmArgs& args) {
   using C = Cfg<BN>;
+  constexpr bool kTma = KIND != KIND_GENERAL;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + C::kStages * C::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  uint8_t* sStore = smem + C::kStages * C::kStageBytes;  // 1024-byte aligned: the swizzled staging layout needs it
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sStore + C::kStoreBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + C::kStages;
-  uint8_t* sStore = smem + C::kStages * C::kStageBytes + C::kBarBytes;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -108,7 +239,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (args.tma_store) tma_prefetch_desc(&tmC);
+    if (kTma) tma_prefetch_desc(&tmC);
     for (int s = 0; s < C::kStages; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], kConsumerWarps);  // every consumer warp releases the slot once its own MMAs have read it
@@ -143,8 +274,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;               // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
     const int wrow = wg * 64 + (warp & 3) * 16;  // first of this warp's 16 rows
-    const int quad = lane & 3;
-    const bool swiglu = args.act == ACT_SWIGLU;
     uint8_t* my_store = sStore + warp * 2048;
     int sbuf = 0;
     int stage = 0;
@@ -174,107 +303,44 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wgmma_wait<0>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
 
-      // ---- epilogue: this thread holds rows r[0], r[1] = r[0] + 8 and, per 8-column group, 2 adjacent columns
-      int row[2];
-      long out_row[2];
-      int grp_row[2] = {0, 0};
-      bool row_ok[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        row[h] = tm * BM + wrow + (lane >> 2) + h * 8;
-        row_ok[h] = row[h] < args.M;
-        out_row[h] = row[h];
-        if (args.rows_per_group > 0) {
-          grp_row[h] = row[h] % args.rows_per_group;
-          out_row[h] = (long)(row[h] / args.rows_per_group) * args.group_stride + grp_row[h] + args.group_offset;
+      // ---- epilogue: one compile-time kind per branch, chosen once per tile (block-uniform)
+#define N1_EPI(act, tma) epilogue<BN, act, tma>(acc, args, &tmC, tm, tn, wrow, lane, my_store, sbuf)
+      if constexpr (KIND == KIND_LINEAR_SWIGLU) {
+        if (args.act == ACT_SWIGLU) N1_EPI(ACT_SWIGLU, true);
+        else N1_EPI(ACT_NONE, true);
+      } else if constexpr (KIND == KIND_GENERAL) {
+        switch (args.act) {
+          case ACT_GELU: N1_EPI(ACT_GELU, false); break;
+          case ACT_RELU: N1_EPI(ACT_RELU, false); break;
+          case ACT_SWIGLU: N1_EPI(ACT_SWIGLU, false); break;
+          case ACT_GELU_TANH: N1_EPI(ACT_GELU_TANH, false); break;
+          case ACT_SILU: N1_EPI(ACT_SILU, false); break;
+          default: N1_EPI(ACT_NONE, false); break;
         }
+      } else {
+        N1_EPI(KIND, true);
       }
-#pragma unroll
-      for (int chunk = 0; chunk < BN / 32; ++chunk) {  // unrolled: the accumulator is indexed statically
-        const int col0 = tn * BN + chunk * 32;
-        if (col0 >= args.N) break;  // block-uniform
-        float v[4][4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = col0 + j * 8 + quad * 2;
-          const bool col_ok = col < args.N;
-#pragma unroll
-          for (int e = 0; e < 4; ++e) v[j][e] = acc[(chunk * 4 + j) * 4 + e];
-          if (args.bias && col_ok) {
-            const float2 b = __ldg(reinterpret_cast<const float2*>(args.bias + col));
-            v[j][0] += b.x, v[j][1] += b.y, v[j][2] += b.x, v[j][3] += b.y;
-          }
-          if (swiglu) {  // (gate, up) interleaved: this thread's column pair -> one output
-            v[j][0] = silu(v[j][0]) * v[j][1];
-            v[j][2] = silu(v[j][2]) * v[j][3];
-            continue;
-          }
-#pragma unroll
-          for (int e = 0; e < 4; ++e) v[j][e] = apply_act(v[j][e], args.act);
-          if (args.gamma && col_ok) {
-            const float2 g = __ldg(reinterpret_cast<const float2*>(args.gamma + col));
-            v[j][0] *= g.x, v[j][1] *= g.y, v[j][2] *= g.x, v[j][3] *= g.y;
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (!row_ok[h] || !col_ok) continue;
-            if (args.row_add) {
-              const float2 a = __ldg(reinterpret_cast<const float2*>(args.row_add + (long)grp_row[h] * args.N + col));
-              v[j][2 * h] += a.x, v[j][2 * h + 1] += a.y;
-            }
-            if (args.residual) {
-              const uint32_t q = __ldg(reinterpret_cast<const uint32_t*>(args.residual + out_row[h] * args.ldr + col));
-              v[j][2 * h] += bf16_lo(q), v[j][2 * h + 1] += bf16_hi(q);
-            }
-          }
-        }
-        if (args.tma_store) {
-          // 16 rows x 32 columns (SwiGLU: 16 output columns) staged per warp, then one bulk tensor store
-          if (lane == 0) tma_store_wait_read<1>();
-          __syncwarp();
-          uint8_t* sb = my_store + sbuf * 1024;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = (lane >> 2) + h * 8;
-              if (swiglu)
-                *reinterpret_cast<bf16*>(sb + r * 32 + (j * 4 + quad) * 2) = __float2bfloat16_rn(v[j][2 * h]);
-              else
-                *reinterpret_cast<uint32_t*>(sb + r * 64 + (j * 8 + quad * 2) * 2) = pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
-            }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            // rows >= M / cols >= N are clipped by the tensor map
-            tma_store_2d(&tmC, sb, swiglu ? col0 >> 1 : col0, tm * BM + wrow);
-            tma_store_commit();
-          }
-          sbuf ^= 1;
-          continue;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = col0 + j * 8 + quad * 2;
-          if (col >= args.N) continue;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (!row_ok[h]) continue;
-            if (swiglu)
-              reinterpret_cast<bf16*>(args.out)[out_row[h] * args.ldo + (col >> 1)] = __float2bfloat16_rn(v[j][2 * h]);
-            else if (args.out_fp32)
-              *reinterpret_cast<float2*>(reinterpret_cast<float*>(args.out) + out_row[h] * args.ldo + col) =
-                  make_float2(v[j][2 * h], v[j][2 * h + 1]);
-            else
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(args.out) + out_row[h] * args.ldo + col) =
-                  pack_bf16(v[j][2 * h], v[j][2 * h + 1]);
-          }
-        }
-      }
+#undef N1_EPI
     }
-    if (args.tma_store && lane == 0) tma_store_wait<0>();
+    if (kTma && lane == 0) tma_store_wait<0>();
     __syncwarp();
   }
+}
+
+// The linear and SwiGLU kinds: every System-2 GEMM but the merger's first layer.
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const GemmArgs args) {
+  gemm_body<BN, KIND_LINEAR_SWIGLU>(tmA, tmB, tmC, args);
+}
+
+// One activation per instance (KIND = ACT_GELU / ACT_RELU / ACT_GELU_TANH / ACT_SILU), or KIND_GENERAL.
+template <int BN, int KIND>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_act_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmC, const GemmArgs args) {
+  gemm_body<BN, KIND>(tmA, tmB, tmC, args);
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -296,8 +362,10 @@ EncodeTiledFn encode_fn() {
 }
 
 // 2-D bf16 tensor map over a row-major [rows, cols] matrix with leading dimension ld; box = [box_rows, box_cols];
-// operands use box_cols = 64 with the 128-byte swizzle, output staging tiles are unswizzled.
-CUtensorMap make_map(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols = BK, bool swizzle = true) {
+// operands use box_cols = 64 with the 128-byte swizzle, output staging tiles the 64-byte (32 columns) or 32-byte
+// (SwiGLU's 16 columns) one.
+CUtensorMap make_map(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols = BK,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   N1_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "GEMM operand not 16-byte aligned");
   N1_CHECK(ld % 8 == 0, "GEMM operand leading dimension must be a multiple of 8 elements");
   CUtensorMap m;
@@ -306,18 +374,25 @@ CUtensorMap make_map(const bf16* ptr, long rows, long cols, long ld, int box_row
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<bf16*>(ptr), gdim, gstr, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw Error(-5, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
   return m;
 }
 
-template <int BN>
+template <int BN, int KIND>
+constexpr auto kernel_of() {
+  if constexpr (KIND == KIND_LINEAR_SWIGLU) return gemm_kernel<BN>;
+  else return gemm_act_kernel<BN, KIND>;
+}
+
+template <int BN, int KIND>
 void launch(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, GemmArgs& a, cudaStream_t stream) {
   using C = Cfg<BN>;
+  auto* kernel = kernel_of<BN, KIND>();
   static std::once_flag once;
-  std::call_once(once, [] {
-    cudaFuncSetAttribute(gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+  std::call_once(once, [kernel] {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
   });
   a.tiles_m = (M + BM - 1) / BM;
   a.tiles_n = (N + BN - 1) / BN;
@@ -335,15 +410,29 @@ void launch(const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K,
   }
   CUtensorMap tmA = make_map(A, M, K, lda, BM);
   CUtensorMap tmB = make_map(W, N, K, ldw, BN);
-  CUtensorMap tmC = tmA;  // placeholder when the direct-store epilogue is used
-  if (a.tma_store) {
+  CUtensorMap tmC = tmA;  // placeholder for the direct-store epilogue (KIND_GENERAL)
+  if (KIND != KIND_GENERAL) {
     const bool sw = a.act == ACT_SWIGLU;
-    tmC = make_map(static_cast<const bf16*>(a.out), M, sw ? N / 2 : N, a.ldo, 16, sw ? 16 : 32, false);
+    tmC = make_map(static_cast<const bf16*>(a.out), M, sw ? N / 2 : N, a.ldo, 16, sw ? 16 : 32,
+                   sw ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B);
   }
   const int tiles = a.tiles_m * a.tiles_n;
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-  gemm_kernel<BN><<<grid, kThreads, C::kSmemBytes, stream>>>(tmA, tmB, tmC, a);
+  kernel<<<grid, kThreads, C::kSmemBytes, stream>>>(tmA, tmB, tmC, a);
   N1_CUDA(cudaGetLastError());
+}
+
+template <int BN>
+void launch_kind(int kind, const bf16* A, int lda, const bf16* W, int ldw, int M, int N, int K, GemmArgs& a,
+                 cudaStream_t stream) {
+  switch (kind) {
+    case KIND_LINEAR_SWIGLU: return launch<BN, KIND_LINEAR_SWIGLU>(A, lda, W, ldw, M, N, K, a, stream);
+    case ACT_GELU: return launch<BN, ACT_GELU>(A, lda, W, ldw, M, N, K, a, stream);
+    case ACT_RELU: return launch<BN, ACT_RELU>(A, lda, W, ldw, M, N, K, a, stream);
+    case ACT_GELU_TANH: return launch<BN, ACT_GELU_TANH>(A, lda, W, ldw, M, N, K, a, stream);
+    case ACT_SILU: return launch<BN, ACT_SILU>(A, lda, W, ldw, M, N, K, a, stream);
+    default: return launch<BN, KIND_GENERAL>(A, lda, W, ldw, M, N, K, a, stream);
+  }
 }
 
 // ---- profiling state
@@ -366,7 +455,7 @@ std::vector<ShapeAcc> g_shapes;  // per-(M, N, K) sums of the event-timed launch
 }  // namespace
 
 CUtensorMap tma_map_2d(const bf16* ptr, long rows, long cols, long ld, int box_rows, int box_cols, bool swizzle) {
-  return make_map(ptr, rows, cols, ld, box_rows, box_cols, swizzle);
+  return make_map(ptr, rows, cols, ld, box_rows, box_cols, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 CUtensorMap tma_map_3d_sw128(const bf16* ptr, const long dims[3], const long strides[2], const int box[3]) {
   N1_CHECK((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && strides[0] % 8 == 0 && strides[1] % 8 == 0,
@@ -471,7 +560,15 @@ void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ld
   a.act = e.act, a.out_fp32 = e.out_fp32;
   a.rows_per_group = e.rows_per_group, a.group_stride = e.group_stride, a.group_offset = e.group_offset;
   a.row_add = e.row_add;
-  a.tma_store = (!e.out_fp32 && e.rows_per_group == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && ldo % 8 == 0) ? 1 : 0;
+  // bf16 output tiles leave through smem staging and TMA stores (full-sector writes) wherever a tensor map can describe
+  // the output; the activation then picks the kernel instance, and everything else takes the general direct-store path
+  const bool tma = !e.out_fp32 && e.rows_per_group == 0 && !e.row_add && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
+                   ldo % 8 == 0;
+  int kind = KIND_GENERAL;
+  if (tma) {
+    kind = KIND_LINEAR_SWIGLU;  // also an act value outside GemmAct, which the epilogue has always treated as none
+    if (e.act == ACT_GELU || e.act == ACT_RELU || e.act == ACT_GELU_TANH || e.act == ACT_SILU) kind = e.act;
+  }
   // Tile-width choice from the shape and the SM count: the least waves x (BN + fixed prologue / epilogue share), ties to
   // the wider tile (fewer A re-reads, longer MMA bursts).  The 256-wide tile is a candidate only when W does not fit the
   // L2 (the raster rule's test in launch()): there the 128-wide tile is held back by operand traffic and 256 wins (LLM
@@ -492,9 +589,9 @@ void gemm_bf16(const bf16* A, int lda, const bf16* W, int ldw, void* out, int ld
   const double flops = 2.0 * M * (double)N * K;
   const int ticket = prof_begin(flops, M, N, K, stream);
   prof_count_gemm(flops);
-  if (bn == 256) launch<256>(A, lda, W, ldw, M, N, K, a, stream);
-  else if (bn == 128) launch<128>(A, lda, W, ldw, M, N, K, a, stream);
-  else launch<64>(A, lda, W, ldw, M, N, K, a, stream);
+  if (bn == 256) launch_kind<256>(kind, A, lda, W, ldw, M, N, K, a, stream);
+  else if (bn == 128) launch_kind<128>(kind, A, lda, W, ldw, M, N, K, a, stream);
+  else launch_kind<64>(kind, A, lda, W, ldw, M, N, K, a, stream);
   prof_end(ticket, stream);
 }
 
