@@ -328,6 +328,10 @@ int n1_op_attention_bwd(const void* q, const void* k, const void* v, const void*
  * internvla_n1_policy.py L212-214).  Reference constants: turn 15 deg (pass np.deg2rad(15)), step 0.25 m, lookahead 4. */
 int n1_traj_to_actions(const void* traj_f32, int B, int Ns, int T, double turn_angle_rad, double step_size, int lookahead,
                        int max_actions, int cap, int32_t* ids, int32_t* count, double* mean_path, void* stream);
+/* The waypoint tail of the real-world agent (vln_utils.py `traj_to_actions(..., use_discrate_action=False)`, called at
+ * internvla_n1_agent_realworld.py L162): n1_traj_to_actions's mean path alone, no walk.  traj fp32 [B * Ns, T, 3] ->
+ * mean_path double [B, T + 1, 2], bit-equal to numpy's in-place `/ 4`, float32 cumsum and float64 mean. */
+int n1_traj_mean_path(const void* traj_f32, int B, int Ns, int T, double* mean_path, void* stream);
 /* C[M,N] (+)= op(A) op(B), fp32 row-major (trans_a: A stored [K,M]; trans_b: B stored [N,K]): the 3-wide and fp32-only
  * products of the training step (action embedding / head, navdp.py L79, L186; position-table resample, dinov2.py L180-211) */
 int n1_op_sgemm(const void* A_f32, int lda, int trans_a, const void* B_f32, int ldb, int trans_b, void* C_f32, int ldc, int M,

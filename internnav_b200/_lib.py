@@ -142,6 +142,7 @@ SYMBOLS = {
     "n1_rgb_tokens": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]),
     "n1_traj_to_actions": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double, c_int, c_int, c_int,
                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+    "n1_traj_mean_path": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "n1_prof_enable": (None, [c_int]),
     "n1_prof_add": (None, [ctypes.c_int64, ctypes.c_int64]),
     "n1_prof_read": (c_int, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),

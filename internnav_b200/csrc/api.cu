@@ -569,6 +569,9 @@ int n1_traj_to_actions(const void* traj, int B, int Ns, int T, double turn_angle
                     count, mean_path, S(stream));
   });
 }
+int n1_traj_mean_path(const void* traj, int B, int Ns, int T, double* mean_path, void* stream) {
+  return guard([&] { traj_mean_path(static_cast<const float*>(traj), B, Ns, T, mean_path, S(stream)); });
+}
 int n1_op_sgemm(const void* A, int lda, int trans_a, const void* B, int ldb, int trans_b, void* C, int ldc, int M, int N, int K,
                 int accumulate, void* stream) {
   return guard([&] {

@@ -166,5 +166,7 @@ void cfg_euler(const bf16* pred, int ld, long n, int cfg, float scale, float dt,
 // walk produced; may exceed cap), optional mean path double [B, T + 1, 2].  max_actions > 0: stop once that many ids exist.
 void traj_to_actions(const float* traj, int B, int Ns, int T, double turn_rad, double step_size, int lookahead,
                      int max_actions, int cap, int* ids, int* count, double* mean_out, cudaStream_t s);
+// the mean path alone (traj_to_actions without the walk): mean_out double [B, T + 1, 2]
+void traj_mean_path(const float* traj, int B, int Ns, int T, double* mean_out, cudaStream_t s);
 
 }  // namespace n1

@@ -41,7 +41,7 @@ __device__ __forceinline__ double normalize_angle(double a) {
 }
 
 // one block per environment; blockDim = 64 * ceil(...): threads (sample, channel) build the cumulative sums, threads
-// (t, channel) the mean, thread 0 walks the path.
+// (t, channel) the mean, thread 0 walks the path.  ids == NULL: the mean path alone (mean_out), no walk.
 __global__ void traj_actions_kernel(const float* __restrict__ traj, int Ns, int T, double turn_rad, double step_size,
                                     int lookahead, int max_actions, int cap, int* __restrict__ ids,
                                     int* __restrict__ count, double* __restrict__ mean_out) {
@@ -68,6 +68,7 @@ __global__ void traj_actions_kernel(const float* __restrict__ traj, int Ns, int 
     mean[i] = m;
     if (mean_out) mean_out[(size_t)env * (T + 1) * 2 + i] = m;
   }
+  if (ids == nullptr) return;
   __syncthreads();
   if (tid != 0) return;
   int n = 0;
@@ -107,9 +108,8 @@ __global__ void traj_actions_kernel(const float* __restrict__ traj, int Ns, int 
 
 }  // namespace
 
-void traj_to_actions(const float* traj, int B, int Ns, int T, double turn_rad, double step_size, int lookahead,
-                     int max_actions, int cap, int* ids, int* count, double* mean_out, cudaStream_t s) {
-  N1_CHECK(traj && ids && count && B > 0 && Ns > 0 && T > 0 && cap > 0, "traj_to_actions: bad arguments");
+static void launch_traj_kernel(const float* traj, int B, int Ns, int T, double turn_rad, double step_size, int lookahead,
+                               int max_actions, int cap, int* ids, int* count, double* mean_out, cudaStream_t s) {
   const size_t smem = ((size_t)Ns * (T + 1) * 2 + (size_t)(T + 1) * 2) * sizeof(double);
   N1_CHECK(smem <= 200 * 1024, "traj_to_actions: Ns * (T + 1) too large for shared memory");
   static size_t attr = 48 * 1024;
@@ -120,6 +120,17 @@ void traj_to_actions(const float* traj, int B, int Ns, int T, double turn_rad, d
   traj_actions_kernel<<<B, 64, smem, s>>>(traj, Ns, T, turn_rad, step_size, lookahead, max_actions, cap, ids, count, mean_out);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
+}
+
+void traj_to_actions(const float* traj, int B, int Ns, int T, double turn_rad, double step_size, int lookahead,
+                     int max_actions, int cap, int* ids, int* count, double* mean_out, cudaStream_t s) {
+  N1_CHECK(traj && ids && count && B > 0 && Ns > 0 && T > 0 && cap > 0, "traj_to_actions: bad arguments");
+  launch_traj_kernel(traj, B, Ns, T, turn_rad, step_size, lookahead, max_actions, cap, ids, count, mean_out, s);
+}
+
+void traj_mean_path(const float* traj, int B, int Ns, int T, double* mean_out, cudaStream_t s) {
+  N1_CHECK(traj && mean_out && B > 0 && Ns > 0 && T > 0, "traj_mean_path: bad arguments");
+  launch_traj_kernel(traj, B, Ns, T, 0.0, 0.0, 0, 0, 0, nullptr, nullptr, mean_out, s);
 }
 
 }  // namespace n1

@@ -104,6 +104,21 @@ def batched_traj_to_actions(dp_actions, num_envs, use_discrate_action=True, max_
     return out
 
 
+def batched_traj_to_waypoints(dp_actions, num_envs):
+    """dp_actions [num_envs * Ns, T, 3] (not modified) -> float64 numpy [num_envs, T + 1, 2]: per environment the mean path
+    that `traj_to_actions(..., use_discrate_action=False)` returns (the real-world agent's System-1 output, vln_utils.py
+    L127-133), bit-equal to it.  CUDA tensors take the kernel (n1_traj_mean_path; D2H = the paths); host tensors numpy."""
+    assert dp_actions.dim() == 3 and dp_actions.shape[2] == 3 and dp_actions.shape[0] % num_envs == 0
+    if not dp_actions.is_cuda:
+        return np.stack(batched_traj_to_actions(dp_actions, num_envs, use_discrate_action=False))
+    from . import _lib
+    t = dp_actions.detach().float().contiguous()
+    ns, T = t.shape[0] // num_envs, t.shape[1]
+    mean = torch.empty(num_envs, T + 1, 2, dtype=torch.float64, device=t.device)
+    _lib.check(_lib.lib().n1_traj_mean_path(_lib.ptr(t), num_envs, ns, T, _lib.ptr(mean), _lib.stream_ptr()))
+    return mean.cpu().numpy()
+
+
 def chunk_token(dp_actions):
     out_list = []
     for i in range(len(dp_actions)):
