@@ -180,17 +180,18 @@ class InternVLAN1Policy:
         return out
 
     # ------------------------------------------------------------------ System 2
-    def _build_inputs(self, ep, rgb, instruction, look_down):
+    def _build_inputs(self, ep, rgb, instruction, look_down, conjunction=CONJUNCTION):
         """L113-164 for one environment -> processor output (input_ids [1, S], pixel_values, image_grid_thw)."""
         image = Image.fromarray(rgb).convert("RGB")
         if not look_down:
             image = image.resize((self.resize_w, self.resize_h))
-        chat = self._chat(ep, image, instruction, look_down)
+        chat = self._chat(ep, image, instruction, look_down, conjunction)
         return self.processor(text=[chat], images=ep.input_images, return_tensors="pt")
 
-    def _chat(self, ep, image, instruction, look_down):
+    def _chat(self, ep, image, instruction, look_down, conjunction=CONJUNCTION):
         """L113-163 for one environment: records the (resized, unless look_down) frame and extends the conversation ->
-        the chat text, one image placeholder per image of ep.input_images."""
+        the chat text, one image placeholder per image of ep.input_images.  `conjunction` opens the sentence that shows
+        the current frame."""
         if not look_down:
             ep.rgb_list.append(image)
             ep.conversation_history = []
@@ -209,7 +210,7 @@ class InternVLAN1Policy:
             assert ep.llm_output != "", "Last llm_output should not be empty when look down"
             text = ""
             ep.conversation_history.append({"role": "assistant", "content": [{"type": "text", "text": ep.llm_output}]})
-        text += " %s." % (CONJUNCTION + DEFAULT_IMAGE_TOKEN)
+        text += " %s." % (conjunction + DEFAULT_IMAGE_TOKEN)
         content = []
         for part in split_and_clean(copy.deepcopy(text)):
             if part == DEFAULT_IMAGE_TOKEN:
@@ -228,14 +229,14 @@ class InternVLAN1Policy:
         merge2 = QwenImagePreprocessor.MERGE ** 2
         return parts[0] + "".join(tok * (int(t * h * w) // merge2) + p for (t, h, w), p in zip(grids.tolist(), parts[1:]))
 
-    def _prepare_device(self, env_ids, rgbs, instructions, look_downs, results):
+    def _prepare_device(self, env_ids, rgbs, instructions, look_downs, conjunctions, results):
         """The device path of s2_step's input preparation -> (prepared [(j, input_ids list)], device bf16 pixel rows,
         image_grid_thw); per-environment failures go to results[j]."""
         frames = self._device_frames(rgbs, [not ld for ld in look_downs])
         chats = []
-        for j, (e, ins, ld) in enumerate(zip(env_ids, instructions, look_downs)):
+        for j, (e, ins, ld, cj) in enumerate(zip(env_ids, instructions, look_downs, conjunctions)):
             try:
-                chats.append((j, self._chat(self.episodes[e], frames[j], ins, ld)))
+                chats.append((j, self._chat(self.episodes[e], frames[j], ins, ld, cj)))
             except Exception as exc:  # noqa: BLE001 -- reported per environment; the agent applies the retry rule
                 results[j] = exc
         if not chats:
@@ -249,21 +250,24 @@ class InternVLAN1Policy:
             g += n
         return prepared, pixels, grids
 
-    def s2_step(self, env_ids, rgbs, depths, poses, instructions, intrinsic, look_downs):
+    def s2_step(self, env_ids, rgbs, depths, poses, instructions, intrinsic, look_downs, conjunctions=None):
         """One System-2 consultation for the listed environments (one model call).  Returns a list with, per
         environment, an S2Output (discrete `output_action` list, or `output_pixel` + `output_latent` [1, n_query, H];
-        None without a System 1) or the Exception that environment's host-side preparation raised."""
+        None without a System 1) or the Exception that environment's host-side preparation raised.  `conjunctions`:
+        per environment, the phrase before the current frame's placeholder (default "you can see ", as this policy's
+        reference does; the VLN-CE evaluator draws one at random per call)."""
         results = [None] * len(env_ids)
+        conjunctions = [CONJUNCTION] * len(env_ids) if conjunctions is None else list(conjunctions)
         if self._vl is not None:
-            prepared, pixels, grids = self._prepare_device(env_ids, rgbs, instructions, look_downs, results)
+            prepared, pixels, grids = self._prepare_device(env_ids, rgbs, instructions, look_downs, conjunctions, results)
             if not prepared:
                 return results
             prompts = [ids for _, ids in prepared]
         else:
             prepared = []
-            for j, (e, rgb, ins, ld) in enumerate(zip(env_ids, rgbs, instructions, look_downs)):
+            for j, (e, rgb, ins, ld, cj) in enumerate(zip(env_ids, rgbs, instructions, look_downs, conjunctions)):
                 try:
-                    prepared.append((j, self._build_inputs(self.episodes[e], rgb, ins, ld)))
+                    prepared.append((j, self._build_inputs(self.episodes[e], rgb, ins, ld, cj)))
                 except Exception as exc:  # noqa: BLE001 -- reported per environment; the agent applies the retry rule
                     results[j] = exc
             if not prepared:
