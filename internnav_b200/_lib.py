@@ -360,17 +360,44 @@ def attention_varlen(q, k, v, heads_q, heads_kv, head_dim, cu_seqlens, max_seq, 
     return o, bool(used.value)
 
 
+ATTN_KERNELS = {1: "short", 2: "generic", 3: "wgmma"}
+
+
+def attention_test(q, k, v, o, heads_q, heads_kv, head_dim, batch, seq_q=0, seq_k=0, cu_q=None, cu_k=None, max_seq_q=0,
+                   kv_div=1, causal=False, scale=None, k_len=None, k_slot=0, k_row0=None, total_rows=0):
+    """attention() with every AttnParams field into a caller-owned view `o` (q / k / v / o: views with unit inner stride;
+    cu_q / cu_k / k_len / k_row0 int32 device tensors or None) -> the kernel that ran, as reported by the library's
+    routing rule: ("short", 48, 16-key tiles, sequences per CTA), ("generic", head dim, 0, 1) or ("wgmma", 128, 0, 1).
+    For tests: n1_test_attention is exported but is not part of include/n1b200.h."""
+    for t in (q, k, v, o):
+        assert t.dtype == torch.bfloat16 and t.stride(1) == 1
+    fn = lib().n1_test_attention
+    fn.restype = c_int
+    fn.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                   c_int, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_float, c_void_p, c_int, c_void_p,
+                   ctypes.c_int64, c_void_p, c_void_p]
+    route = (c_int * 4)()
+    vp = lambda t: c_void_p(t.data_ptr())
+    check(fn(vp(q), vp(k), vp(v), vp(o), q.stride(0), k.stride(0), v.stride(0), o.stride(0), heads_q, heads_kv, head_dim,
+             batch, seq_q, seq_k, ptr(cu_q), ptr(cu_k), int(max_seq_q), kv_div, 1 if causal else 0,
+             float(head_dim ** -0.5 if scale is None else scale), ptr(k_len), int(k_slot), ptr(k_row0), int(total_rows),
+             route, stream_ptr()))
+    return ATTN_KERNELS[route[0]], route[1], route[2], route[3]
+
+
 def attention_cache(q, k, v, heads_q, heads_kv, cu_q, ctx, row0, max_chunk, scale=None, out=None):
     """Chunk attention over a slotted K/V cache (head_dim 128): q [rows, >=heads_q*128] packed chunk rows (sequence b at
     cu_q[b] .. cu_q[b + 1]), k / v [kv_rows, heads_kv*128] cache rows (sequence b's keys at row0[b] .. row0[b] + ctx[b] +
-    n_b - 1), cu_q / ctx / row0 int32 device tensors -> o [rows, heads_q*128] bf16, bottom-right causal."""
+    n_b - 1), cu_q / ctx / row0 int32 device tensors -> o [rows, heads_q*128] bf16, bottom-right causal.  `out` may be
+    a view with a wider row stride."""
     assert q.dtype == k.dtype == v.dtype == torch.bfloat16 and q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1
     assert k.stride(0) == v.stride(0) and k.shape[0] == v.shape[0]
     for t in (cu_q, ctx, row0):
         assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
     o = torch.empty(q.shape[0], heads_q * 128, device=q.device, dtype=torch.bfloat16) if out is None else out
+    assert o.dtype == torch.bfloat16 and o.stride(1) == 1 and o.is_cuda
     check(lib().n1_op_attention_cache(c_void_p(q.data_ptr()), q.stride(0), q.shape[0], c_void_p(k.data_ptr()),
-                                      c_void_p(v.data_ptr()), k.stride(0), k.shape[0], ptr(o), o.stride(0), ptr(cu_q),
+                                      c_void_p(v.data_ptr()), k.stride(0), k.shape[0], c_void_p(o.data_ptr()), o.stride(0), ptr(cu_q),
                                       ptr(ctx), ptr(row0), cu_q.numel() - 1, int(max_chunk), heads_q, heads_kv,
                                       float(128 ** -0.5 if scale is None else scale), stream_ptr()))
     return o

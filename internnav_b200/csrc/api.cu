@@ -774,6 +774,29 @@ int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int
   });
 }
 
+// Test entry point, deliberately not declared in include/n1b200.h: attention() with every AttnParams field (var-len,
+// kv_div sharing, the slotted K/V cache's k_len / k_slot / k_row0, total_rows), reporting the kernel attention_route()
+// picked in route[4] = {kernel (1 short-sequence, 2 generic, 3 wgmma), head dim, short kernel's 16-key tiles, its query
+// sequences per CTA}.
+int n1_test_attention(const void* q, const void* k, const void* v, void* o, int ldq, int ldk, int ldv, int ldo, int heads_q,
+                      int heads_kv, int head_dim, int batch, int seq_q, int seq_k, const int32_t* cu_q, const int32_t* cu_k,
+                      int max_seq_q, int kv_div, int causal, float scale, const int32_t* k_len, int k_slot,
+                      const int32_t* k_row0, int64_t total_rows, int* route, void* stream) {
+  return guard([&] {
+    if (!route) throw Error(N1_ERR_ARG, "n1_test_attention: null route");
+    AttnParams p = {};
+    p.q = B16(q), p.k = B16(k), p.v = B16(v), p.o = B16(o);
+    p.ldq = ldq, p.ldk = ldk, p.ldv = ldv, p.ldo = ldo;
+    p.heads_q = heads_q, p.heads_kv = heads_kv, p.hd = head_dim, p.batch = batch;
+    p.seq_q = seq_q, p.seq_k = seq_k, p.cu_q = cu_q, p.cu_k = cu_k, p.max_seq_q = max_seq_q;
+    p.kv_div = kv_div, p.causal = causal, p.scale = scale;
+    p.k_len = k_len, p.k_slot = k_slot, p.k_row0 = k_row0, p.total_rows = total_rows;
+    const AttnRoute r = attention_route(p);
+    route[0] = r.kernel, route[1] = r.hd, route[2] = r.nkp, route[3] = r.group;
+    attention(p, S(stream));
+  });
+}
+
 int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
                           void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
                           int max_chunk, int heads_q, int heads_kv, float scale, void* stream) {

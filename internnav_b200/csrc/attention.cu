@@ -302,7 +302,7 @@ __global__ void __launch_bounds__(256) attn_small_kernel(const AttnParams p, con
 }
 
 template <int NKP>
-void launch_attn_small(const AttnParams& p, cudaStream_t stream) {
+void launch_attn_small(const AttnParams& p, int G, cudaStream_t stream) {
   const int RS = p.heads_q * 96 + 16;
   const int smem = (((p.seq_q + 15) & ~15) + 2 * NKP * 16) * RS;
   static bool attr_set = false;
@@ -310,9 +310,6 @@ void launch_attn_small(const AttnParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(attn_small_kernel<NKP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (32 + 2 * NKP * 16) * (8 * 96 + 16));
     attr_set = true;
   }
-  int G = 1;  // sequences per CTA: only when they share K/V
-  if (p.kv_div % 4 == 0 && p.batch % 4 == 0) G = 4;
-  else if (p.kv_div % 2 == 0 && p.batch % 2 == 0) G = 2;
   attn_small_kernel<NKP><<<p.batch / G, p.heads_q * 32, smem, stream>>>(p, G);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
@@ -345,6 +342,22 @@ bool attention_uses_tc(const AttnParams& p) {
   return tc != 0;
 }
 
+AttnRoute attention_route(const AttnParams& p) {
+  AttnRoute r = {ATTN_GENERIC, p.hd, 0, 1};
+  if (p.hd == 48 && !p.cu_q && !p.cu_k && !p.k_len && p.heads_q == p.heads_kv && p.heads_q <= 8 && p.seq_q <= 32 && p.seq_k <= 64 &&
+      p.ldo % 8 == 0) {
+    const int nkp = (p.seq_k + 15) / 16;
+    r.kernel = ATTN_SHORT;
+    r.nkp = nkp >= 1 && nkp <= 3 ? nkp : 4;
+    // sequences per CTA: only when they share K/V
+    if (p.kv_div % 4 == 0 && p.batch % 4 == 0) r.group = 4;
+    else if (p.kv_div % 2 == 0 && p.batch % 2 == 0) r.group = 2;
+  } else if (attention_uses_tc(p)) {
+    r.kernel = ATTN_WGMMA;
+  }
+  return r;
+}
+
 void attention(const AttnParams& p, cudaStream_t stream) {
   if (p.batch <= 0) return;
   N1_CHECK(p.heads_kv > 0 && p.heads_q % p.heads_kv == 0, "attention: heads_q must be a multiple of heads_kv");
@@ -352,16 +365,15 @@ void attention(const AttnParams& p, cudaStream_t stream) {
   N1_CHECK(p.ldq % 8 == 0 && p.ldk % 8 == 0 && p.ldv % 8 == 0 && p.ldo % 2 == 0, "attention: misaligned strides");
   N1_CHECK(!p.cu_q || p.max_seq_q > 0, "attention: varlen needs max_seq_q");
   N1_CHECK(p.batch <= 65535 && p.heads_q <= 65535, "attention: grid too large");
-  if (p.hd == 48 && !p.cu_q && !p.cu_k && !p.k_len && p.heads_q == p.heads_kv && p.heads_q <= 8 && p.seq_q <= 32 && p.seq_k <= 64 &&
-      p.ldo % 8 == 0) {
-    const int nkp = (p.seq_k + 15) / 16;
-    if (nkp == 1) launch_attn_small<1>(p, stream);
-    else if (nkp == 2) launch_attn_small<2>(p, stream);
-    else if (nkp == 3) launch_attn_small<3>(p, stream);
-    else launch_attn_small<4>(p, stream);
+  const AttnRoute r = attention_route(p);
+  if (r.kernel == ATTN_SHORT) {
+    if (r.nkp == 1) launch_attn_small<1>(p, r.group, stream);
+    else if (r.nkp == 2) launch_attn_small<2>(p, r.group, stream);
+    else if (r.nkp == 3) launch_attn_small<3>(p, r.group, stream);
+    else launch_attn_small<4>(p, r.group, stream);
     return;
   }
-  if (attention_uses_tc(p)) {
+  if (r.kernel == ATTN_WGMMA) {
     attention_tc128(p, stream);
     return;
   }

@@ -106,6 +106,15 @@ struct AttnParams {
                          //   sequence that lives in a slot of a caller-owned K/V pool)
 };
 void attention(const AttnParams& p, cudaStream_t stream);
+// The kernel attention(p) runs: the one routing rule, which attention() dispatches on and n1_test_attention reports.
+enum AttnKernel { ATTN_SHORT = 1, ATTN_GENERIC = 2, ATTN_WGMMA = 3 };
+struct AttnRoute {
+  int kernel;  // AttnKernel
+  int hd;      // head dim of the kernel instance
+  int nkp;     // short-sequence kernel: 16-key tiles (1..4); 0 otherwise
+  int group;   // short-sequence kernel: query sequences per CTA (1, 2 or 4); 1 otherwise
+};
+AttnRoute attention_route(const AttnParams& p);
 // wgmma / TMA attention for head_dim 128, var-len self-attention with <= 320 keys per sequence (attention_wgmma.cu)
 bool attention_tc_supported(const AttnParams& p);
 // whether attention(p) runs the wgmma kernel: supported arguments and not disabled by N1_ATTN_TC=0

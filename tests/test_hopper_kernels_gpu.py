@@ -207,9 +207,24 @@ def wgrad_splits(M, No, Ko, sms):
 
 # ------------------------------------------------------------------------------------------ attention decoys
 HD = 128
-DECOY_UNIT_NATS = 8.0            # one score unit = 64 raw (q . k) at scale 1/8
-DECOY_SCALE = DECOY_UNIT_NATS / 64.0
-_PARITY = 16                     # units: own-sequence keys -16, next-sequence keys +16, TMA's zero rows 0
+DECOY_UNIT_NATS = 8.0            # one score unit = P raw (q . k) at scale 8 / P
+# Key code per head dim: a P-Hadamard row on key % P, a one-hot (value P) on key // P, one parity column (the last).
+# hd -> P; hd - P - 1 block columns, so a sequence of up to P (hd - P - 1) keys is exact (480 / 992 / 960 / 4032).
+DECOY_P = {48: 32, 64: 32, 80: 64, 128: 64}
+_PARITY = 16                     # units: own-sequence keys -16, opposite-parity keys +16, zero rows 0
+
+
+def decoy_scale(hd=HD):
+    return DECOY_UNIT_NATS / DECOY_P[hd]
+
+
+def decoy_max_keys(hd=HD):
+    """Longest key sequence the decoy code keeps exact at this head dim."""
+    P = DECOY_P[hd]
+    return P * (hd - P - 1)
+
+
+DECOY_SCALE = decoy_scale(HD)    # 1/8
 
 
 def _hadamard(n):
@@ -219,136 +234,186 @@ def _hadamard(n):
     return h
 
 
-def decoy_targets(i, n, causal, hq):
-    """Target key of query row i (sequence length n) for query head hq: key 0, the diagonal, the last key of every 64-key
-    block, the key one block back and one spread key, rotated by row and head so each head of a group sees others."""
-    lim = i if causal else n - 1
-    cands = sorted({0, min(i, lim), max(i - 64, 0), (i * 5 + 3) % (lim + 1)} | {b for b in range(63, lim + 1, 64)})
-    return cands[(i * 3 + hq) % len(cands)]
+def decoy_candidates(pos, lim):
+    """Target candidates of a query row whose diagonal key is `pos` and whose last visible key is `lim`: key 0, the
+    diagonal, the key one 64-key tile back, one spread key and the last key of every 64-key tile."""
+    return sorted({0, min(pos, lim), min(max(pos - 64, 0), lim), (pos * 5 + 3) % (lim + 1)} | set(range(63, lim + 1, 64)))
 
 
-def decoy_query(i, n, t, causal, sigma):
-    """Score units per key code for row i with target t -> (A [64] by key % 64, B [6] by key // 64, parity weight).
+def decoy_key_code(n, sigma, hd=HD):
+    """[n, hd] key code of keys 0 .. n - 1 of one sequence with parity sigma (+-1)."""
+    P = DECOY_P[hd]
+    assert n <= decoy_max_keys(hd), "sequence of %d keys is past the exact decoy limit at hd %d" % (n, hd)
+    j = torch.arange(n)
+    code = torch.zeros(n, hd)
+    code[:, :P] = _hadamard(P)[j % P]
+    code[j, P + j // P] = float(P)
+    code[:, hd - 1] = -float(P) * sigma
+    return code
 
-    Own-sequence key j scores A[j % 64] + B[j // 64] - 16 units.  Non-causal: target 6, every other key <= 3.  Causal:
-    target 12, every visible key <= 9, and where the row can take one, an in-block decoy at key i + 1 scores 15; every
-    key of a later 64-key block scores >= 15.  Keys of the next sequence score >= +16 and zero rows 0.  So the target
-    beats every visible key by >= 3 units (24 nats), and those decoys beat the target by >= 3 units."""
-    A, B = [0] * 64, [0] * 6
-    ia, ib, ta, tb = i % 64, i // 64, t % 64, t // 64
+
+def decoy_query_code(sq, sk, causal, sigma, hq, hd=HD):
+    """Query code of a sequence of sq query rows over sk keys (bottom-right causal: row i sees keys j <= i + sk - sq, so a
+    chunk at offset ctx into its keys is sq = n, sk = ctx + n) -> (q [sq, hq, hd], target key per (row, head) [sq, hq]).
+
+    In score units (own-sequence key j scores A[j % P] + B[j // P] - 16): non-causal, the target 6 and every other key
+    <= 3.  Causal, the target 12 and every visible key <= 9; where the row can take one, an in-block decoy at key i + 1
+    scores 15, and every key of a later P-key block scores >= 15.  Keys of the opposite parity score >= +16 and zero rows
+    0.  So the target beats every visible key by >= 3 units (24 nats), and those decoys beat the target by >= 3 units.
+    Targets rotate over the candidates by row and head, so each head of a GQA group sees others."""
+    P = DECOY_P[hd]
+    nb = hd - P - 1
+    assert sk <= decoy_max_keys(hd) and (not causal or sq <= sk)
+    pos = np.arange(sq) + (sk - sq if causal else 0)
+    lim = pos if causal else np.full(sq, sk - 1)
+    heads = np.arange(hq)
+    # decoy_candidates for every row at once: sorted, duplicates pushed to the end, then picked by (pos * 3 + head)
+    big = np.iinfo(np.int64).max
+    ends = 63 + 64 * np.arange(max(int(lim.max()) + 1, 0) // 64)
+    c = np.concatenate((np.stack((np.zeros(sq, np.int64), np.minimum(pos, lim), np.minimum(np.maximum(pos - 64, 0), lim),
+                                  (pos * 5 + 3) % (lim + 1)), 1),
+                        np.where(ends[None, :] <= lim[:, None], ends[None, :], big)), 1)
+    c.sort(1)
+    c[:, 1:][c[:, 1:] == c[:, :-1]] = big
+    c.sort(1)
+    count = (c != big).sum(1)
+    t = np.take_along_axis(c, (pos[:, None] * 3 + heads[None, :]) % count[:, None], 1)
+    A = np.zeros((sq, hq, P), dtype=np.float32)
+    B = np.zeros((sq, hq, nb), dtype=np.float32)
+    r, h = np.arange(sq)[:, None], heads[None, :]
+    ta, tb = t % P, t // P
     if not causal:
-        A[ta], B[tb] = 3, 3
+        A[r, h, ta], B[r, h, tb] = 3, 3
     else:
-        decoy = i + 1 < n and ia < 63
-        if tb == ib:
-            A[ta], B[ib] = 3, 9
-            if decoy:
-                A[ia + 1] = 6
-        else:
-            A[ta], B[tb] = 9, 3
-            if decoy and ta > ia + 1:   # key (ta, ib) is then hidden too, and A[ia + 1] is not the target's
-                A[ia + 1], B[ib] = 6, 9
-        for fb in range(ib + 1, (n + 63) // 64):
-            B[fb] = 15
-    return A, B, _PARITY * sigma
+        ia, ib = np.broadcast_to((pos % P)[:, None], t.shape), np.broadcast_to((pos // P)[:, None], t.shape)
+        decoy = np.broadcast_to(((pos + 1 < sk) & (pos % P < P - 1))[:, None], t.shape)
+        same = tb == ib
+        A[r, h, ta] = np.where(same, 3, 9)
+        B[r, h, tb] = np.where(same, 9, 3)
+        d = decoy & (same | (ta > ia + 1))   # other block: key (ta, ib) is then hidden too, and A[ia + 1] not the target's
+        rr, hh = np.nonzero(d)
+        A[rr, hh, ia[rr, hh] + 1] = 6
+        B[rr, hh, ib[rr, hh]] = 9
+        later = (np.arange(nb)[None, None, :] > ib[:, :, None]) & (np.arange(nb)[None, None, :] < (sk + P - 1) // P)
+        B[later] = 15
+    q = torch.zeros(sq, hq, hd)
+    q[:, :, :P] = torch.from_numpy(A) @ _hadamard(P)
+    q[:, :, P:P + nb] = torch.from_numpy(B)
+    q[:, :, hd - 1] = _PARITY * sigma
+    return q, torch.from_numpy(t)
 
 
-def make_decoy_attention(lens, hkv, group, causal, seed=0, device="cpu", tail_rows=320):
-    """q, k, v bf16 buffers of sum(lens) + tail_rows rows (the rows past the end hold decoys the kernel must never load)
-    and the expected output: row i of head h is exactly V[target(i, h)] of the head's K-V head."""
+def decoy_values(rows, cols, gen):
+    """V entries: integers of magnitude 1 .. 8 with random signs."""
+    return small_ints((rows, cols), 1, 8, gen, torch.float32) * (small_ints((rows, cols), 0, 1, gen, torch.float32) * 2 - 1)
+
+
+def decoy_expect(v, key_rows, group, hd=HD):
+    """Expected output [rows, hq * hd]: row r of head h is V[key_rows[r, h]] of K-V head h // group."""
+    hq = key_rows.shape[1]
+    kv_cols = (torch.arange(hq) // group)[:, None] * hd + torch.arange(hd)[None, :]
+    return v.cpu()[key_rows[:, :, None], kv_cols[None, :, :]].reshape(key_rows.shape[0], hq * hd)
+
+
+def make_decoy_attention(lens, hkv, group, causal, seed=0, device="cpu", tail_rows=320, hd=HD):
+    """Packed var-len decoys: q, k, v bf16 buffers of sum(query lengths) / sum(key lengths) + tail_rows rows (the rows
+    past the end hold decoys the kernel must never load) and the expected output: row i of head h is exactly
+    V[target(i, h)] of the head's K-V head.  An entry of `lens` is n (n queries over n keys) or (sq, sk).
+    Consecutive sequences alternate parity.  -> (q, k, v, expect, targets as rows of k)."""
     hq_total = hkv * group
-    T = sum(lens)
-    H64 = _hadamard(64)
+    P = DECOY_P[hd]
+    pairs = [(n, n) if isinstance(n, int) else tuple(n) for n in lens]
+    Tq, Tk = sum(sq for sq, _ in pairs), sum(sk for _, sk in pairs)
     gen = torch.Generator().manual_seed(seed)
-    q = torch.zeros(T + tail_rows, hq_total * HD)
-    k = torch.zeros(T + tail_rows, hkv * HD)
-    v = small_ints((T + tail_rows, hkv * HD), 1, 8, gen, torch.float32) * (small_ints((T + tail_rows, hkv * HD), 0, 1, gen,
-                                                                                       torch.float32) * 2 - 1)
-    targets = np.zeros((T, hq_total), dtype=np.int64)
-    A = np.zeros((T, hq_total, 64), dtype=np.float32)
-    B = np.zeros((T, hq_total, 6), dtype=np.float32)
-    par = np.zeros((T, hq_total), dtype=np.float32)
-    start = 0
-    for b, n in enumerate(lens):
+    q = torch.zeros(Tq + tail_rows, hq_total, hd)
+    k = torch.zeros(Tk + tail_rows, hkv, hd)
+    v = decoy_values(Tk + tail_rows, hkv * hd, gen)
+    targets = torch.zeros(Tq, hq_total, dtype=torch.int64)
+    qs = ks = 0
+    for b, (sq, sk) in enumerate(pairs):
         sigma = 1 if b % 2 == 0 else -1
-        j = torch.arange(n)
-        code = torch.zeros(n, HD)
-        code[:, :64] = H64[j % 64]
-        code[j, 64 + j // 64] = 64.0
-        code[:, 70] = -64.0 * sigma
-        for kh in range(hkv):
-            k[start:start + n, kh * HD:(kh + 1) * HD] = code
-        for i in range(n):
-            for h in range(hq_total):
-                t = decoy_targets(i, n, causal, h)
-                A[start + i, h], B[start + i, h], par[start + i, h] = decoy_query(i, n, t, causal, sigma)
-                targets[start + i, h] = start + t
-        start += n
-    targets = torch.from_numpy(targets)
-    qv = q.view(T + tail_rows, hq_total, HD)
-    qv[:T, :, :64] = torch.from_numpy(A) @ H64
-    qv[:T, :, 64:70] = torch.from_numpy(B)
-    qv[:T, :, 70] = torch.from_numpy(par)
+        k[ks:ks + sk] = decoy_key_code(sk, sigma, hd)[:, None, :]
+        q[qs:qs + sq], t = decoy_query_code(sq, sk, causal, sigma, hq_total, hd)
+        targets[qs:qs + sq] = ks + t
+        qs, ks = qs + sq, ks + sk
     # rows past the end: every block code and no parity, so they beat any target if they were ever loaded
-    k[T:, 64:70] = 64.0
-    q, k, v = (x.to(torch.bfloat16).to(device) for x in (q, k, v))
+    k[Tk:, :, P:hd - 1] = float(P)
+    q, k, v = (x.reshape(x.shape[0], -1).to(torch.bfloat16).to(device) for x in (q, k, v))
+    return q, k, v, decoy_expect(v, targets, group, hd).to(device), targets
+
+
+def attention_ref_rows(q, k, v, seqs, hkv, group, scale, hd=HD, head_map=None):
+    """float64 attention sequence by sequence: seqs = [(q_rows [n], k_rows [m], vis [n])] with q_rows rows of q,
+    k_rows rows of k / v (-1: a zero row) and keys [0, vis[i]) of k_rows visible to query row i; GQA head h on K-V head
+    head_map(h) (default h // group).  -> (out, mag = sum p |v| / sum p, dlogit = bound on the fp32 logit error (nats)),
+    each over the concatenated q_rows."""
+    hq_total = hkv * group
+    dev = q.device
     heads = torch.arange(hq_total)
-    kv_cols = (heads // group)[:, None] * HD + torch.arange(HD)[None, :]               # [hq, HD]
-    expect = v.cpu()[targets[:, :, None], kv_cols[None, :, :]].reshape(T, hq_total * HD)
-    return q, k, v, expect.to(device), targets
+    kvh = (head_map(heads) if head_map is not None else heads // group).to(dev)
+    zero = lambda x: torch.cat((x.double(), torch.zeros(1, x.shape[1], dtype=torch.float64, device=dev)))
+    k64 = zero(k).view(-1, k.shape[1] // hd, hd)[:, :hkv]
+    v64 = zero(v).view(-1, v.shape[1] // hd, hd)[:, :hkv]
+    outs, mags, dls = [], [], []
+    for q_rows, k_rows, vis in seqs:
+        q_rows, k_rows, vis = (torch.as_tensor(x, dtype=torch.int64, device=dev) for x in (q_rows, k_rows, vis))
+        n, m = q_rows.numel(), k_rows.numel()
+        k_rows = torch.where(k_rows < 0, torch.full_like(k_rows, k64.shape[0] - 1), k_rows)
+        qs = q[q_rows].double().view(n, -1, hd)[:, :hq_total].transpose(0, 1)              # [hq, n, hd]
+        kw = k64[k_rows][:, kvh].transpose(0, 1)                                            # [hq, m, hd]
+        vw = v64[k_rows][:, kvh].transpose(0, 1)
+        j = torch.arange(m, device=dev)[None, :]
+        hide = j >= vis[:, None]
+        s = (qs @ kw.transpose(1, 2) * scale).masked_fill(hide, float("-inf"))
+        sabs = (qs.abs() @ kw.abs().transpose(1, 2) * scale).masked_fill(hide, 0.0)
+        p = torch.softmax(s, -1)
+        outs.append((p @ vw).transpose(0, 1).reshape(n, -1))
+        mags.append((p @ vw.abs()).transpose(0, 1).reshape(n, -1))
+        # fp32 Q K^T over hd products, then s * scale * log2(e) - m * scale * log2(e) and ex2.approx (2 ulp)
+        sl = s.masked_fill(hide, 0.0).abs()
+        d = (hd + 8) * U32 * sabs.amax(-1) + 8 * U32 * sl.amax(-1) * math.log2(math.e) + 4 * U32
+        dls.append(d.transpose(0, 1))
+    return torch.cat(outs), torch.cat(mags), torch.cat(dls)
 
 
-def attention_ref(q, k, v, lens, hkv, group, causal, scale, shift=0, window=320):
+def attention_ref(q, k, v, lens, hkv, group, causal, scale, shift=0, window=320, hd=HD):
     """float64 attention over what the wgmma kernel loads: for each sequence the `window` rows from its start (rows past
     the tensor read as zeros, as TMA fills them), keys [0, visible + shift) of it, GQA head h on K-V head h // group.
-    -> (out [T, Hq * HD], mag [T, Hq * HD] = sum p |v| / sum p, dlogit [T, Hq] = bound on the fp32 logit error (nats))."""
-    hq_total = hkv * group
+    -> (out [T, Hq * hd], mag [T, Hq * hd] = sum p |v| / sum p, dlogit [T, Hq] = bound on the fp32 logit error (nats))."""
     T = sum(lens)
     dev = q.device
-    q64, k64, v64 = q[:T].double(), k[:T].double(), v[:T].double()
-    kpad = torch.cat((k64, torch.zeros(window, k64.shape[1], dtype=torch.float64, device=dev)))
-    vpad = torch.cat((v64, torch.zeros(window, v64.shape[1], dtype=torch.float64, device=dev)))
-    out = torch.zeros(T, hq_total * HD, dtype=torch.float64, device=dev)
-    mag = torch.zeros_like(out)
-    dlogit = torch.zeros(T, hq_total, dtype=torch.float64, device=dev)
-    start = 0
+    seqs, start = [], 0
     for n in lens:
-        qs = q64[start:start + n].view(n, hq_total, HD).transpose(0, 1)                          # [hq, n, HD]
-        kw = kpad[start:start + window].view(window, hkv, HD).transpose(0, 1).repeat_interleave(group, 0)
-        vw = vpad[start:start + window].view(window, hkv, HD).transpose(0, 1).repeat_interleave(group, 0)
-        s = qs @ kw.transpose(1, 2) * scale
-        sabs = qs.abs() @ kw.abs().transpose(1, 2) * scale
-        i = torch.arange(n, device=dev)[:, None]
-        j = torch.arange(window, device=dev)[None, :]
+        i = torch.arange(n, device=dev)
+        rows = start + torch.arange(window, device=dev)
         vis = (torch.minimum(i + 1, torch.tensor(n, device=dev)) if causal else torch.full_like(i, n)) + shift
-        s = s.masked_fill(j >= vis, float("-inf"))
-        p = torch.softmax(s, -1)
-        out[start:start + n] = (p @ vw).transpose(0, 1).reshape(n, -1)
-        mag[start:start + n] = (p @ vw.abs()).transpose(0, 1).reshape(n, -1)
-        # fp32 Q K^T over HD products, then s * scale * log2(e) - m * scale * log2(e) and ex2.approx (2 ulp)
-        sl = s.masked_fill(j >= vis, 0.0).abs()
-        d = ((HD + 8) * U32 * sabs.masked_fill(j >= vis, 0.0).amax(-1) + 8 * U32 * sl.amax(-1) * math.log2(math.e) + 4 * U32)
-        dlogit[start:start + n] = d.transpose(0, 1)
+        seqs.append((start + i, torch.where(rows < T, rows, torch.full_like(rows, -1)), vis))
         start += n
-    return out, mag, dlogit
+    return attention_ref_rows(q[:T], k[:T], v[:T], seqs, hkv, group, scale, hd)
 
 
-def attention_bound(out_ref, mag, dlogit, group_heads):
-    """elementwise_bound for the attention output: P is rounded to bf16 before P V (2^-8 of each p in the numerator but
-    not in the row sum), and a logit error d moves each p by a factor within e^{+-d} in numerator and denominator."""
-    rel = BF16_U + 2.0 * dlogit.repeat_interleave(HD, dim=1)
-    return elementwise_bound(out_ref, mag, 320, extra=rel * mag)
+def attention_bound(out_ref, mag, dlogit, group_heads, hd=HD, keys=320):
+    """elementwise_bound for the attention output over `keys` keys: P is rounded to bf16 before P V (2^-8 of each p in
+    the numerator but not in the row sum), and a logit error d moves each p by a factor within e^{+-d} in numerator and
+    denominator."""
+    rel = BF16_U + 2.0 * dlogit.repeat_interleave(hd, dim=1)
+    return elementwise_bound(out_ref, mag, keys, extra=rel * mag)
 
 
-def identify_key(row, v, start, kh, window=320):
-    """Which loaded key's V row (of K-V head kh) the output row equals: for failure messages."""
+def identify_key(row, v, start, kh, window=320, hd=HD, rows=None):
+    """Which loaded key's V row (of K-V head kh) the output row equals: for failure messages.  The candidates are the
+    `window` rows from `start`, or the given `rows` of v (a sequence's keys, in order)."""
     T = v.shape[0]
-    cand = v[start:min(start + window, T), kh * HD:(kh + 1) * HD].float()
+    if rows is None:
+        rows = torch.arange(start, min(start + window, T))
+    cand = v[torch.as_tensor(rows, device=v.device), kh * hd:(kh + 1) * hd].float()
     hit = (cand == row.float()[None, :]).all(1).nonzero()
     if hit.numel():
-        return "key %d of the load window (row %d)" % (int(hit[0]), start + int(hit[0]))
+        return "key %d of the load window (row %d)" % (int(hit[0]), int(rows[int(hit[0])]))
     if bool((row.float() == 0).all()):
         return "a zero row (past the end of the tensor)"
+    if bool(torch.isnan(row.float()).any()):
+        return "NaN (a row the kernel must not read)"
     return "no single key (a mixture)"
 
 

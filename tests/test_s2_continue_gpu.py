@@ -1,6 +1,6 @@
-"""Continuing a System-2 conversation on its K/V cache (the policy's look-down turn), on the GPU: the chunk attention
-kernel against a float64 reference, and the continued generate against the fp32 oracle and the library's own full
-re-prefill."""
+"""Continuing a System-2 conversation on its K/V cache (the policy's look-down turn), on the GPU: the continued generate
+against the fp32 oracle and the library's own full re-prefill.  The chunk attention kernel itself is tested in
+tests/test_attention_paths_gpu.py."""
 import numpy as np
 import pytest
 import torch
@@ -13,45 +13,6 @@ MARGIN = 0.15  # logit units, as tests/test_s2_gpu.py: bf16 near-ties of the gre
 def _rel(a, b):
     a, b = a.float().cpu(), b.float().cpu()
     return ((a - b).norm() / (b.norm() + 1e-12)).item()
-
-
-# ------------------------------------------------------------------------------------------------ kernel
-@pytest.mark.parametrize("ctx", [0, 1, 64, 319, 320, 321, 2047])
-@pytest.mark.parametrize("n", [1, 63, 64, 65, 400])
-def test_attention_cache_vs_fp64(ctx, n):
-    from internnav_b200 import _lib
-    hq, hk, hd = 28, 4, 128
-    g = torch.Generator().manual_seed(1000 * ctx + n)
-    # sequence 0 is the case under test; sequence 1 a shorter one in the same launch; slots permuted
-    seqs = [(ctx, n), (ctx // 3, max(1, n // 2))]
-    slots, cap = [2, 0], ctx + n + 64
-    kv_rows = 3 * cap
-    K = torch.full((kv_rows, hk * hd), float("nan"), dtype=torch.bfloat16)  # rows past k_len must never be read
-    V = torch.full((kv_rows, hk * hd), float("nan"), dtype=torch.bfloat16)
-    qs = []
-    for (c, m), s in zip(seqs, slots):
-        K[s * cap:s * cap + c + m] = torch.randn(c + m, hk * hd, generator=g).bfloat16()
-        V[s * cap:s * cap + c + m] = torch.randn(c + m, hk * hd, generator=g).bfloat16()
-        qs.append(torch.randn(m, hq * hd, generator=g).bfloat16())
-    q = torch.cat(qs)
-    cu = torch.tensor([0, seqs[0][1], seqs[0][1] + seqs[1][1]], dtype=torch.int32)
-    ctx_t = torch.tensor([c for c, _ in seqs], dtype=torch.int32)
-    row0 = torch.tensor([s * cap for s in slots], dtype=torch.int32)
-    o = _lib.attention_cache(q.cuda(), K.cuda(), V.cuda(), hq, hk, cu.cuda(), ctx_t.cuda(), row0.cuda(),
-                             max(m for _, m in seqs))
-    torch.cuda.synchronize()
-    o = o.cpu()
-    assert torch.isfinite(o.float()).all()
-    for b, ((c, m), s) in enumerate(zip(seqs, slots)):
-        qb = q[cu[b]:cu[b + 1]].double().view(m, hq, hd)
-        kb = K[s * cap:s * cap + c + m].double().view(c + m, hk, hd).repeat_interleave(hq // hk, dim=1)
-        vb = V[s * cap:s * cap + c + m].double().view(c + m, hk, hd).repeat_interleave(hq // hk, dim=1)
-        sc = torch.einsum("qhd,khd->hqk", qb, kb) / hd ** 0.5
-        mask = torch.arange(c + m)[None, :] > (c + torch.arange(m))[:, None]
-        sc = sc.masked_fill(mask[None], float("-inf"))
-        ref = torch.einsum("hqk,khd->qhd", sc.softmax(-1), vb).reshape(m, hq * hd)
-        e = _rel(o[cu[b]:cu[b + 1]], ref)
-        assert e < 1e-2, (b, c, m, e)
 
 
 # ------------------------------------------------------------------------------------------------ two-turn conversation
