@@ -40,7 +40,31 @@ Deviations from the reference loop:
     environment's episode; its dict holds `get_metrics()` at that point, the exception's type name under "error" and its
     message under "error_message" (so every dict stays JSON-serialisable), and the other environments carry on;
   * `depth_filter` is supplied by the caller (the reference calls `depth_camera_filtering.filter_depth`).
-The evaluator's `system2` mode needs the simulator's ShortestPathFollower and is not mirrored.
+
+`HabitatVLNEvaluator(mode="system2").run_system2(envs)` mirrors the evaluator's other mode, `_run_eval_system2`
+(L631-945), the benchmark loop of the System-2-only checkpoint, in the same way (`_episodes_system2`):
+
+  * there is no look-down view on every step: the camera tilts only when System 2 answers "↓" (LOOKDOWN twice, no
+    step counted, the conversation kept), and the next call is the look-down turn on the full-size frame; every other
+    environment step clears the conversation (L877-885);
+  * a pixel answer [c0, c1] is the image point (u, v) = (c0, c1): the camera steps LOOKUP twice, the point is lifted
+    with that iteration's depth (filter, affine, `* 1000`, `/ 1000`) through the intrinsics and a camera pose built from
+    gps, compass, the camera height plus the agent's height change and a 30 degree pitch (`pixel_to_gps`, L706-719 /
+    L804), taken to the world frame by the episode-start agent pose and snapped to the navmesh unless navigable
+    (L806-809) -- float64 numpy, the reference's operations in its order;
+  * the caller's ShortestPathFollower then walks to that goal: on the pixel-goal iteration `get_next_action` is called
+    twice (a STOP on the first steps LEFT, drops the goal and clears the conversation); after that once per step, and
+    more than MAX_STEPS calls or a STOP drop the goal and count a step without an environment step, so the next
+    iteration shows System 2 the same observation, which enters the history again (L811-848).
+
+`run_system2` serves every waiting environment in ONE `s2_step` per round, on `generate` alone (`system2_only`: no
+latent pass, whatever the model carries).  Its deviations are those above, plus two:
+  * depth is filtered only when a pixel answer needs it (the reference filters every frame and uses the result only
+    there; the filter is a function of the one frame, so the goals are the same);
+  * a pixel answer the reference cannot use -- a lone number (IndexError at L797) or a point outside the depth frame
+    (IndexError in `pixel_to_gps`) -- and a look-down turn whose conversation an action step of the same answer has
+    cleared (e.g. "←↓": the reference sends one image placeholder with all of the conversation's images, which
+    Qwen2.5-VL refuses) end that environment's episode with `error` / `error_message`.
 """
 import random
 
@@ -56,6 +80,8 @@ S1_SIZE = 224
 MAX_STEPS, MAX_LOCAL_STEPS = 8, 4
 STOP, FORWARD, LEFT, RIGHT, LOOKUP, LOOKDOWN = range(6)
 DEPTH_CLIP = 5.0
+CAMERA_PITCH = np.deg2rad(30)      # the pitch the system2 loop assumes for every pixel answer (L718)
+FOLLOWER_RADIUS = 0.25             # ShortestPathFollower(sim, 0.25, False), once per episode (L663)
 CONJUNCTIONS = ["you can see ", "in front of you is ", "there is ", "you can spot ", "you are toward the ",
                 "ahead of you is ", "in your sight is "]
 
@@ -83,6 +109,78 @@ def summarize(results):
     return out
 
 
+# ---------------------------------------------------------------------------------------------- system2 geometry
+# Float64 numpy in the operations, shapes and order of the reference's internnav/habitat_extensions/vln/utils.py
+# (get_intrinsic_matrix, xyz_yaw_pitch_to_tf_matrix, get_axis_align_matrix, pixel_to_gps), so that every goal is the
+# reference's bit for bit.
+AXIS_ALIGN = np.array([[0, 0, 1, 0], [-1, 0, 0, 0], [0, -1, 0, 0], [0, 0, 0, 1]])
+
+
+def rotation_matrix(q):
+    """numpy-quaternion's `as_rotation_matrix` for one quaternion (w, x, y, z attributes, as habitat's agent rotation
+    has, or a scalar-first 4-sequence) -> float64 [3, 3]; a non-unit quaternion is divided by its squared norm."""
+    w, x, y, z = (q.w, q.x, q.y, q.z) if hasattr(q, "w") else tuple(q)
+    w, x, y, z = float(w), float(x), float(y), float(z)
+    n = w * w + x * x + y * y + z * z
+    if n == 0.0:
+        raise ZeroDivisionError("rotation quaternion has zero norm")
+    return np.array([[1.0 - 2 * (y * y + z * z) / n, 2 * (x * y - z * w) / n, 2 * (x * z + y * w) / n],
+                     [2 * (x * y + z * w) / n, 1.0 - 2 * (x * x + z * z) / n, 2 * (y * z - x * w) / n],
+                     [2 * (x * z - y * w) / n, 2 * (y * z + x * w) / n, 1.0 - 2 * (x * x + y * y) / n]])
+
+
+def agent_to_world(state):
+    """The episode-start agent pose (rotation quaternion, position) as a float64 [4, 4] transform (L655-661)."""
+    m = np.eye(4)
+    m[:3, :3] = rotation_matrix(state.rotation)
+    m[:3, 3] = state.position
+    return m
+
+
+def intrinsic_matrix(width, height, hfov):
+    """Pinhole intrinsics [4, 4] of a width x height sensor with horizontal field of view `hfov` degrees (square
+    pixels, principal point at the centre of the pixel grid)."""
+    f = (width / 2.0) / np.tan(np.deg2rad(hfov / 2.0))
+    return np.array([[f, 0.0, (width - 1.0) / 2.0, 0.0], [0.0, f, (height - 1.0) / 2.0, 0.0],
+                     [0.0, 0.0, 1.0, 0.0], [0.0, 0.0, 0.0, 1.0]])
+
+
+def camera_to_episodic(xyz, yaw, pitch=CAMERA_PITCH):
+    """Camera -> episodic frame [4, 4]: yaw about z, then pitch about y, at position xyz, times the axis alignment that
+    takes the camera's (right, down, forward) axes to (forward, left, up)."""
+    x, y, z = xyz
+    c, s, cp, sp = np.cos(yaw), np.sin(yaw), np.cos(pitch), np.sin(pitch)
+    yaw_m = np.array([[c, -s, 0, x], [s, c, 0, y], [0, 0, 1, z], [0, 0, 0, 1]])[:3, :3]
+    pitch_m = np.array([[cp, 0, sp, x], [0, 1, 0, y], [-sp, 0, cp, z], [0, 0, 0, 1]])[:3, :3]
+    m = np.eye(4)
+    m[:3, :3] = yaw_m @ pitch_m
+    m[:3, 3] = xyz
+    return m @ AXIS_ALIGN
+
+
+def pixel_to_gps(pixel, depth, intrinsic, tf_camera_to_episodic):
+    """Image point pixel = (v, u) with depth[v, u] metres -> its (x, y) in the episodic frame.  A point outside the
+    depth frame raises IndexError."""
+    v, u = pixel
+    z = depth[v, u]
+    p = np.array([(u - intrinsic[0, 2]) * z / intrinsic[0, 0], (v - intrinsic[1, 2]) * z / intrinsic[1, 1], z, 1.0])
+    p = tf_camera_to_episodic @ p
+    p = p[:3] / p[3]
+    return p[0], p[1]
+
+
+def follower_action(a):
+    """A ShortestPathFollower answer (tensor, array or int) as the action the loop steps (L831-832)."""
+    if isinstance(a, torch.Tensor):
+        a = a.detach().cpu().numpy()[0]
+    return a[0] if hasattr(a, "__len__") else a
+
+
+def _shortest_path_follower(env):
+    from habitat.tasks.nav.shortest_path_follower import ShortestPathFollower
+    return ShortestPathFollower(env._env.sim, FOLLOWER_RADIUS, False)
+
+
 class _Request:
     """What one environment waits for: System 2 ("s2": frame, look_down, instruction, conjunction) or System 1 ("s1":
     the look-down frame and its raw depth, `goal` when this frame becomes the pixel-goal frame)."""
@@ -107,14 +205,33 @@ class _Env:
 class HabitatVLNEvaluator:
     def __init__(self, model, processor, num_history=8, resize_w=384, resize_h=384, min_depth=0.0, max_depth=10.0,
                  max_steps_per_episode=500, depth_filter=None, vision_cache_frames=0, seeds=None, x_init=None,
-                 max_new_tokens=128):
+                 max_new_tokens=128, mode="dual_system", camera_height=None, width=640, height=480, hfov=79,
+                 make_follower=None):
         """`depth_filter(depth [H, W], blur_type=None)`: the filter the reference applies to every depth frame; needed
-        only by a System 1 that reads depth.  `seeds`: one `random.Random` seed per environment for the conjunction
-        draws, as many as `run_dual_system` gets environments (default 0, 1, ...).  `x_init`: None (System 1 draws its noise on the device) or a callable env_ids ->
+        by a System 1 that reads depth and by the system2 mode.  `seeds`: one `random.Random` seed per environment for
+        the conjunction draws, as many as `run_*` gets environments (default 0, 1, ...).  `x_init`: None (System 1 draws its noise on the device) or a callable env_ids ->
         initial noise [len(env_ids) * 32, T, 3] for those environments, in that order.  `max_new_tokens`: System 2's
-        answer budget (the reference's 128)."""
-        if not getattr(model, "has_system1", True):
+        answer budget (the reference's 128).
+
+        `mode`: the reference's `model_settings["mode"]`.  "dual_system" (`run_dual_system`) needs a model with a
+        System 1; "system2" (`run_system2`) takes any model with `generate` and also needs the sensor geometry --
+        `camera_height` (metres, the RGB sensor's position[1] in the caller's habitat config; no default), the RGB
+        sensor's `width` x `height` and `hfov` (degrees; vln_r2r.yaml: 640 x 480, 79) and `min_depth` / `max_depth` --
+        and `make_follower(env)`, the per-episode ShortestPathFollower (default: habitat's
+        `ShortestPathFollower(env._env.sim, 0.25, False)`, imported when first needed)."""
+        if mode not in ("dual_system", "system2"):
+            raise ValueError("mode must be 'dual_system' or 'system2', not %r" % (mode,))
+        if mode == "dual_system" and not getattr(model, "has_system1", True):
             raise ValueError("the dual-system evaluation needs a model with a System 1; this one has none")
+        if mode == "system2":
+            if not callable(getattr(model, "generate", None)):
+                raise ValueError("the system2 evaluation needs a model with generate")
+            if camera_height is None:
+                raise ValueError("the system2 evaluation needs camera_height: the RGB sensor's height in the habitat "
+                                 "config")
+            if depth_filter is None:
+                raise ValueError("the system2 evaluation needs depth_filter for the depth of pixel answers")
+        self.mode = mode
         processor.tokenizer.padding_side = "left"
         self.model, self.processor = model, processor
         self.num_history, self.resize_w, self.resize_h = num_history, resize_w, resize_h
@@ -123,11 +240,15 @@ class HabitatVLNEvaluator:
         self.depth_filter, self.vision_cache_frames = depth_filter, vision_cache_frames
         self.seeds, self.x_init, self.max_new_tokens = seeds, x_init, max_new_tokens
         self.device = torch.device(getattr(model, "device", "cpu"))
-        self.reads_depth = getattr(getattr(model, "config", None), "system1", None) == "navdp_async"
+        self.reads_depth = mode == "dual_system" and \
+            getattr(getattr(model, "config", None), "system1", None) == "navdp_async"
         if self.reads_depth and depth_filter is None:
             raise ValueError("a System 1 that reads depth (navdp_async) needs depth_filter")
+        self.camera_height = camera_height
+        self.intrinsic = intrinsic_matrix(width, height, hfov)
+        self.make_follower = _shortest_path_follower if make_follower is None else make_follower
         self._frames = None
-        if self.device.type == "cuda":
+        if self.device.type == "cuda" and mode == "dual_system":
             from .preprocess import FramePreprocessor
             self._frames = FramePreprocessor(self.device, out_size=S1_SIZE)
         self.policy = None
@@ -136,18 +257,28 @@ class HabitatVLNEvaluator:
     # ------------------------------------------------------------------ driver
     def run_dual_system(self, envs):
         """Run every episode of every environment -> per environment the list of its episodes' result dicts."""
+        return self._run("dual_system", envs, self._episodes)
+
+    def run_system2(self, envs):
+        """The system2 mode: run every episode of every environment -> per environment its episodes' result dicts."""
+        return self._run("system2", envs, self._episodes_system2)
+
+    def _run(self, mode, envs, episodes):
+        if mode != self.mode:
+            raise ValueError("run_%s needs an evaluator built with mode=%r; this one has mode=%r" % (mode, mode, self.mode))
         B = len(envs)
         if self.policy is None or len(self.policy.episodes) != B:
             self.policy = P.InternVLAN1Policy(self.model, self.processor, num_envs=B, num_history=self.num_history,
                                               resize_w=self.resize_w, resize_h=self.resize_h,
                                               max_new_tokens=self.max_new_tokens, device=self.device,
-                                              vision_cache_frames=self.vision_cache_frames)
+                                              vision_cache_frames=self.vision_cache_frames,
+                                              system2_only=mode == "system2")
         self.policy.reset()
         seeds = list(range(B)) if self.seeds is None else list(self.seeds)
         if len(seeds) != B:
             raise ValueError("%d seeds for %d environments: give one seed per environment" % (len(seeds), B))
         state = [_Env(s) for s in seeds]
-        gens = [self._episodes(env, st) for env, st in zip(envs, state)]
+        gens = [episodes(env, st, e) for e, (env, st) in enumerate(zip(envs, state))]
         req = {}
         for e, g in enumerate(gens):
             self._advance(req, e, g, None)
@@ -241,7 +372,7 @@ class HabitatVLNEvaluator:
         return t.to(torch.bfloat16)
 
     # ------------------------------------------------------------------ one environment (L271-606)
-    def _episodes(self, env, st):
+    def _episodes(self, env, st, e):
         """The reference loop for one environment; yields a _Request where the reference calls the model and receives
         the S2Output (or Exception) of System 2, or the local action chunk of System 1."""
         while env.is_running:
@@ -307,16 +438,121 @@ class HabitatVLNEvaluator:
                 else:
                     obs, _, done, _ = env.step(action)
                     step_id += 1
-            metrics = env.get_metrics()
-            result = {"scene_id": scene_id, "episode_id": episode_id, "success": metrics["success"],
-                      "spl": metrics["spl"], "os": metrics["oracle_success"], "ne": metrics["distance_to_goal"],
-                      "steps": step_id, "episode_instruction": instruction}
-            if "ndtw" in metrics:
-                result["ndtw"] = metrics["ndtw"]
-            if error is not None:
-                result["error"], result["error_message"] = type(error).__name__, str(error)
-            st.results.append(result)
+            st.results.append(self._result(env, scene_id, episode_id, step_id, instruction, error))
+
+    @staticmethod
+    def _result(env, scene_id, episode_id, step_id, instruction, error):
+        """The episode's progress.json dict (L590-601 / L909-920), plus the error that ended it, if any."""
+        metrics = env.get_metrics()
+        result = {"scene_id": scene_id, "episode_id": episode_id, "success": metrics["success"],
+                  "spl": metrics["spl"], "os": metrics["oracle_success"], "ne": metrics["distance_to_goal"],
+                  "steps": step_id, "episode_instruction": instruction}
+        if "ndtw" in metrics:
+            result["ndtw"] = metrics["ndtw"]
+        if error is not None:
+            result["error"], result["error_message"] = type(error).__name__, str(error)
+        return result
 
     def _own(self, obs):
         """Copies of an observation's RGB frame and, for a System 1 that reads depth, its depth frame (else None)."""
         return np.array(obs["rgb"]), (np.array(obs["depth"]) if self.reads_depth else None)
+
+    # ------------------------------------------------------------------ one environment, system2 mode (L640-935)
+    def _episodes_system2(self, env, st, e):
+        """The reference's system2 loop for environment e; yields a _Request where the reference calls the model and
+        receives the S2Output (or Exception) of System 2."""
+        while env.is_running:
+            obs = env.reset()
+            if not env.is_running or obs is None:
+                break
+            st.history, st.reset = [], True
+            episode = env.get_current_episode()
+            scene_id, episode_id = episode.scene_id.split("/")[-2], int(episode.episode_id)
+            instruction = episode.instruction.instruction_text
+            sim = env._env.sim
+            to_world = agent_to_world(sim.get_agent_state())
+            follower = self.make_follower(env)
+            initial_height = sim.get_agent_state().position[1]
+            step_id, action_seq, action, goal, forward_action = 0, [], None, None, 0
+            talking = False     # the last System-2 conversation is still open: no action step since
+            done, error = False, None
+            # the observation is copied when it arrives: an iteration that takes no step shows the same one again
+            cur = self._own_system2(obs)
+            while not done and step_id <= self.max_steps_per_episode:
+                rgb, depth, gps, compass = cur
+                ask = len(action_seq) == 0 and goal is None
+                if action != LOOKDOWN and not ask:
+                    st.history.append(rgb)   # a System-2 call adds its own frame to the history
+                if ask:
+                    height = sim.get_agent_state().position[1] - initial_height
+                    look_down = action == LOOKDOWN
+                    conjunction = st.rng.choice(CONJUNCTIONS)
+                    if look_down and not talking:
+                        n = len(self.policy.episodes[e].input_images) + 1
+                        error = ValueError("a look-down turn after an action step: the cleared conversation has 1 image "
+                                           "placeholder for %d images" % n)
+                        break
+                    res = yield _Request("s2", rgb, look_down=look_down, instruction=instruction[:-1],
+                                         conjunction=conjunction)
+                    if isinstance(res, Exception):
+                        error = res
+                        break
+                    talking = True
+                    if res.output_pixel is not None:
+                        forward_action = 0
+                        env.step(LOOKUP)
+                        env.step(LOOKUP)
+                        try:
+                            goal = self._world_goal(sim, [int(v) for v in res.output_pixel], depth, gps, compass,
+                                                    height, to_world)
+                        except IndexError as exc:
+                            error = exc
+                            break
+                        if follower.get_next_action(goal) == STOP:
+                            goal, action, talking = None, LEFT, False
+                            obs, _, done, _ = env.step(action)
+                            cur = self._own_system2(obs)
+                            step_id += 1
+                            continue
+                    else:
+                        action_seq = list(res.output_action)
+                if len(action_seq) != 0:
+                    action = action_seq.pop(0)
+                elif goal is not None:
+                    action = follower_action(follower.get_next_action(goal))
+                    forward_action += 1
+                    if forward_action > MAX_STEPS or action == STOP:
+                        goal, forward_action, talking = None, 0, False
+                        step_id += 1
+                        continue
+                else:
+                    action = STOP
+                if action == LOOKDOWN:
+                    env.step(action)
+                    obs, _, done, _ = env.step(action)
+                else:
+                    obs, _, done, _ = env.step(action)
+                    step_id += 1
+                    talking = False
+                cur = self._own_system2(obs)
+            st.results.append(self._result(env, scene_id, episode_id, step_id, instruction, error))
+
+    def _world_goal(self, sim, pixel, depth, gps, compass, height, to_world):
+        """A pixel answer -> its navigable world goal (L710-712, L716-719, L804-809): the depth frame filtered, scaled
+        to metres and lifted through the camera pose of this iteration, then taken to the world frame by the
+        episode-start agent pose and snapped to the navmesh unless navigable."""
+        d = self.depth_filter(depth.reshape(depth.shape[:2]), blur_type=None)
+        d = d * (self.max_depth - self.min_depth) + self.min_depth
+        d = d * 1000
+        x, y = gps
+        tf = camera_to_episodic(np.array([x, -y, self.camera_height + height]), compass[0])
+        g = pixel_to_gps(pixel, d / 1000, self.intrinsic, tf)
+        goal = (to_world @ np.array([-g[1], 0, -g[0], 1]))[:3]
+        if not sim.pathfinder.is_navigable(np.array(goal)):
+            goal = np.array(sim.pathfinder.snap_point(np.array(goal)))
+        return goal
+
+    @staticmethod
+    def _own_system2(obs):
+        """Copies of an observation's RGB, depth, gps and compass."""
+        return np.array(obs["rgb"]), np.array(obs["depth"]), np.array(obs["gps"]), np.array(obs["compass"])

@@ -20,7 +20,8 @@ image and the processor prepares each environment's prompt on the host, as in th
 
 A model without a System 1 (`system1 = None`, the System-2-only checkpoint) is served as the reference evaluator serves it
 in its `system2` mode: `s2_step` calls `generate` alone (no TRAJ pass), pixel answers carry no latent plan
-(`output_latent` is None), and `s1_step_latent` raises.
+(`output_latent` is None), and `s1_step_latent` raises.  `system2_only=True` serves any model that way, one with a System
+1 included: the evaluator's `system2` mode loads the checkpoint as plain Qwen2.5-VL, so no latent plan is ever computed.
 """
 import copy
 import itertools
@@ -87,13 +88,15 @@ class _Episode:
 
 class InternVLAN1Policy:
     def __init__(self, model, processor, num_envs=1, num_history=8, resize_w=384, resize_h=384, continuous_traj=True,
-                 max_new_tokens=128, device=None, vision_cache_frames=0):
+                 max_new_tokens=128, device=None, vision_cache_frames=0, system2_only=False):
         self.model, self.processor = model, processor
         self.num_history, self.resize_w, self.resize_h = num_history, resize_w, resize_h
         self.continuous_traj = continuous_traj
         self.max_new_tokens = max_new_tokens
         self.device = device if device is not None else getattr(model, "device", "cpu")
         self.has_system1 = getattr(model, "has_system1", True)
+        # whether s2_step computes latent plans (generate_with_latents) or calls generate alone
+        self.latent_plans = self.has_system1 and not system2_only
         self.episodes = [_Episode() for _ in range(num_envs)]
         # K/V cache of each environment's last System-2 conversation, passed back on its look-down turn only (the turn
         # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
@@ -253,7 +256,7 @@ class InternVLAN1Policy:
     def s2_step(self, env_ids, rgbs, depths, poses, instructions, intrinsic, look_downs, conjunctions=None):
         """One System-2 consultation for the listed environments (one model call).  Returns a list with, per
         environment, an S2Output (discrete `output_action` list, or `output_pixel` + `output_latent` [1, n_query, H];
-        None without a System 1) or the Exception that environment's host-side preparation raised.  `conjunctions`:
+        None without a System 1 or with system2_only) or the Exception that environment's host-side preparation raised.  `conjunctions`:
         per environment, the phrase before the current frame's placeholder (default "you can see ", as this policy's
         reference does; the VLN-CE evaluator draws one at random per call)."""
         results = [None] * len(env_ids)
@@ -281,7 +284,7 @@ class InternVLAN1Policy:
         if features is not None:
             kw["feature_pool"] = features
         with torch.no_grad():
-            if self.has_system1:
+            if self.latent_plans:
                 out = self.model.generate_with_latents(prompts, pixels, grids, max_new_tokens=self.max_new_tokens, **kw)
             else:
                 out = self.model.generate(prompts, pixels, grids, max_new_tokens=self.max_new_tokens,
@@ -296,7 +299,7 @@ class InternVLAN1Policy:
                 if re.search(r"\d", ep.llm_output):   # pixel goal "y x" -> [x, y] plus the latent plan (L179-190)
                     coord = [int(c) for c in re.findall(r"\d+", ep.llm_output)]
                     res.output_pixel = np.array([int(coord[1]), int(coord[0])])
-                    res.output_latent = out.latents[n:n + 1] if self.has_system1 else None
+                    res.output_latent = out.latents[n:n + 1] if self.latent_plans else None
                 else:
                     res.output_action = parse_actions(ep.llm_output)
                 results[j] = res

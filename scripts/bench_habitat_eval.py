@@ -1,7 +1,8 @@
-"""Throughput of the batched VLN-CE evaluation loop (HabitatVLNEvaluator.run_dual_system) for B environments.
+"""Throughput of the batched VLN-CE evaluation loop (HabitatVLNEvaluator.run_dual_system, or run_system2 with
+`--mode system2`) for B environments.
 
-    python scripts/bench_habitat_eval.py [--batches 1,8,64] [--episodes 2] [--max-steps 24] [--repeats 3] [--max-new 8]
-                                         [--out FILE]
+    python scripts/bench_habitat_eval.py [--mode dual_system|system2] [--batches 1,8,64] [--episodes 2] [--max-steps 24]
+                                         [--repeats 3] [--max-new 8] [--out FILE]
 
 Weights are seeded random at the Qwen2.5-VL-7B shapes with the nextdit_async System 1 (the released DualVLN head);
 frames are 480 x 640, resized to 384 x 384 for System 2 on the device (PIL Qwen2-VL image processor, reproduced by
@@ -17,6 +18,10 @@ timed on the host with a device synchronise after it.  Reported: environment ste
 same episodes also run one environment at a time (eight B = 1 drivers in turn), the reference's one-process-per-
 environment shape, alternating with the batched runs; the ratio of the two rates is reported per repeat.  Card name,
 power limit and SM clock are read in the same run.
+
+`--mode system2` runs the System-2-only model (the same seeded 7B System 2, no System 1) through `run_system2`: the
+synthetic environment also carries a zero-cost simulator surface (agent state, a navmesh that accepts every goal) and
+the follower answers FORWARD three times per goal, then STOP, so every pixel answer is lifted to a world goal and walked.
 """
 import argparse
 import json
@@ -67,6 +72,37 @@ class SyntheticEnv:
         return {"success": 0.0, "spl": 0.0, "oracle_success": 0.0, "distance_to_goal": 1.0, "top_down_map": None}
 
 
+class _Sim:
+    """The zero-cost simulator surface of the system2 loop: a fixed agent state and a navmesh that takes every goal."""
+
+    def __init__(self):
+        from types import SimpleNamespace
+        state = SimpleNamespace(position=np.zeros(3, dtype=np.float32), rotation=SimpleNamespace(w=1.0, x=0.0, y=0.0, z=0.0))
+        self.get_agent_state = lambda: state
+        self.pathfinder = SimpleNamespace(is_navigable=lambda p: True, snap_point=lambda p: p)
+
+
+class SyntheticEnvS2(SyntheticEnv):
+    def __init__(self, *args):
+        super().__init__(*args)
+        from types import SimpleNamespace
+        self._env = SimpleNamespace(sim=_Sim())
+
+    def _obs(self):
+        return dict(super()._obs(), compass=np.zeros(1, dtype=np.float32))
+
+
+class Follower:
+    """FORWARD three times per goal, then STOP."""
+
+    def __init__(self, env):
+        self.n = 0
+
+    def get_next_action(self, goal):
+        self.n += 1
+        return 0 if self.n % 4 == 0 else 1
+
+
 class ScriptedAnswers(BenchProcessor._Tok):
     """Each environment cycles through ANSWERS; answers are told apart by the order of decode calls within a System-2
     call, which follows the order of the environments the evaluator passes (set by `Timed._round`)."""
@@ -82,7 +118,7 @@ class ScriptedAnswers(BenchProcessor._Tok):
         return ANSWERS[n % len(ANSWERS)]
 
 
-def make_evaluator(model, proc, max_steps, max_new):
+def make_evaluator(model, proc, max_steps, max_new, mode="dual_system"):
     from internnav_b200.habitat_eval import HabitatVLNEvaluator
 
     class Timed(HabitatVLNEvaluator):
@@ -94,8 +130,10 @@ def make_evaluator(model, proc, max_steps, max_new):
             torch.cuda.synchronize()
             self.round_ms.append((time.perf_counter() - t0) * 1e3)
 
+    kw = {} if mode == "dual_system" else dict(camera_height=1.25, depth_filter=lambda d, blur_type=None: d,
+                                               make_follower=Follower)
     ev = Timed(model, proc, num_history=8, resize_w=384, resize_h=384, max_steps_per_episode=max_steps,
-               max_new_tokens=max_new)
+               max_new_tokens=max_new, mode=mode, **kw)
     ev.round_ms = []
     return ev
 
@@ -104,10 +142,11 @@ def run(ev, proc, robots, frames, depth, episodes):
     """Run `episodes` episodes on each listed robot's environment -> (env steps, seconds, round times)."""
     ev.robots, ev.round_ms = robots, []
     proc.tokenizer.count = {}
-    envs = [SyntheticEnv(frames[r % len(frames)], depth, r, episodes) for r in robots]
+    system2 = ev.mode == "system2"
+    envs = [(SyntheticEnvS2 if system2 else SyntheticEnv)(frames[r % len(frames)], depth, r, episodes) for r in robots]
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    res = ev.run_dual_system(envs)
+    res = ev.run_system2(envs) if system2 else ev.run_dual_system(envs)
     torch.cuda.synchronize()
     sec = time.perf_counter() - t0
     assert not any("error" in x for rs in res for x in rs), res
@@ -127,6 +166,7 @@ def summary(runs):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--mode", default="dual_system", choices=["dual_system", "system2"])
     ap.add_argument("--batches", default="1,8,64")
     ap.add_argument("--episodes", type=int, default=2)
     ap.add_argument("--max-steps", type=int, default=24)
@@ -142,13 +182,14 @@ def main():
     from internnav_b200.manifest import random_nextdit_state_dict
     from oracle import qwen_oracle as Q
     cfg = dict(Q.QWEN25VL_7B, layers=a.layers)
-    result = {"card": card(), "cfg": dict(layers=a.layers, max_new_tokens=a.max_new, num_history=8, frame="480x640",
+    result = {"card": card(), "cfg": dict(mode=a.mode, layers=a.layers, max_new_tokens=a.max_new, num_history=8, frame="480x640",
                                           resize="384x384", episodes=a.episodes, max_steps_per_episode=a.max_steps,
                                           repeats=a.repeats)}
     print(json.dumps(result), flush=True)
-    model = InternVLAN1ForCausalLM(cfg, device="cuda:0", system1="nextdit_async")
+    system1 = "nextdit_async" if a.mode == "dual_system" else None
+    model = InternVLAN1ForCausalLM(cfg, device="cuda:0", system1=system1)
     s2_sd = Q.make_s2_state_dict(cfg, seed=0, device="cuda", dtype=torch.bfloat16, lm_head=True)
-    model.load_parts(s2_sd, random_nextdit_state_dict(1, device="cuda", dtype=torch.bfloat16))
+    model.load_parts(s2_sd, random_nextdit_state_dict(1, device="cuda", dtype=torch.bfloat16) if system1 else None)
     del s2_sd
     torch.cuda.empty_cache()
     proc = BenchProcessor(Qwen2VLImageProcessorPil(min_pixels=3136, max_pixels=12845056))
@@ -158,12 +199,12 @@ def main():
     depth = np.full((480, 640, 1), 0.3, dtype=np.float32)
     for B in [int(x) for x in a.batches.split(",")]:
         robots = list(range(B))
-        ev = make_evaluator(model, proc, 6, a.max_new)
+        ev = make_evaluator(model, proc, 6, a.max_new, a.mode)
         run(ev, proc, robots, frames, depth, 1)                       # warm-up: 6 steps per environment
         ev.max_steps_per_episode = a.max_steps
         one = None
         if B == 8:
-            one = make_evaluator(model, proc, 6, a.max_new)
+            one = make_evaluator(model, proc, 6, a.max_new, a.mode)
             run(one, proc, [0], frames, depth, 1)
             one.max_steps_per_episode = a.max_steps
         batched, single = [], []
