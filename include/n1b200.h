@@ -297,7 +297,9 @@ int n1_rgb_tokens(n1_handle h, void* ws, size_t ws_bytes, const float* rgb, void
 /* Training branch, System-2 half (internvla_n1.py L128-235 and its backward): `plan` is a generation plan over the
  * prompts WITHOUT the TRAJ tokens (n1_llm_plan_create, max_new_tokens = 1).  Forward: states bf16 [B, n_query, hidden] =
  * hidden states at the TRAJ positions.  Backward: grad_states bf16 [B, n_query, hidden] -> grad_latent_queries fp32
- * [n_query, hidden].  Both calls must be given the SAME workspace (the forward leaves its K/V cache and saves there). */
+ * [n_query, hidden].  Both calls must be given the SAME workspace (the forward leaves its K/V cache and saves there).
+ * A continuation plan (created over a K/V pool) is refused before anything is launched: the workspace size is 0 and
+ * both calls return N1_ERR_ARG. */
 int n1_s2_set_latent_queries(n1_handle h, const void* latent_queries_bf16, void* stream);  /* after an optimizer step */
 size_t n1_s2_train_workspace_bytes(n1_handle h, n1_llm_plan plan);
 int n1_s2_train_forward(n1_handle h, n1_llm_plan plan, void* ws, size_t ws_bytes, const void* image_feats_bf16,

@@ -26,11 +26,6 @@ LNp load_ln(Arena& a, const WeightSource& ws, const std::string& prefix, cudaStr
   return p;
 }
 
-void linear(const Lin& L, const bf16* A, int lda, void* out, int ldo, int M, GemmEpilogue e, cudaStream_t s) {
-  e.bias = L.b;
-  gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
-}
-
 // torch.nn.functional.interpolate(mode="bicubic", scale_factor=s, antialias=False, align_corners=False) restated
 // for the DINOv2 position table (dinov2.py L180-211): [G*G, D] -> [g*g, D] with the *given* scale factor
 // (src = (dst + 0.5) / s - 0.5, A = -0.75, border-clamped taps), fp32 like ATen's upsample_bicubic2d.

@@ -16,6 +16,11 @@ struct Lin {
   float* b = nullptr;  // [N] fp32 or null
   int N = 0, K = 0, ldw = 0;
 };
+// out[M, N] = A[M, K] @ L.w^T with L's bias (if any) in the epilogue
+inline void linear(const Lin& L, const bf16* A, int lda, void* out, int ldo, int M, GemmEpilogue e, cudaStream_t s) {
+  e.bias = L.b;
+  gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
+}
 struct LNp {
   float* w = nullptr;
   float* b = nullptr;

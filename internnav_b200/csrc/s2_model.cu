@@ -25,11 +25,6 @@ T* upload(const std::vector<T>& v, cudaStream_t s) {
   return d;
 }
 
-void linear(const Lin& L, const bf16* A, int lda, void* out, int ldo, int M, GemmEpilogue e, cudaStream_t s) {
-  e.bias = L.b;
-  gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
-}
-
 // [rows_a; rows_b; ...] stacked into one K-major bf16 matrix (+ optional stacked fp32 bias)
 Lin stack_lin(Arena& a, const WeightSource& ws, const std::vector<std::string>& names, bool bias, long cols,
               cudaStream_t s) {
@@ -173,11 +168,11 @@ void S2Model::load(const WeightSource& ws, const S2Dims& d, cudaStream_t s) {
   vblk_.resize(d.v_depth);
   for (int i = 0; i < d.v_depth; ++i) {
     const std::string p = "blocks." + std::to_string(i) + ".";
-    VBlock& b = vblk_[i];
+    Block& b = vblk_[i];
     b.n1 = v.f32(arena_, p + "norm1.weight", s);
     b.n2 = v.f32(arena_, p + "norm2.weight", s);
     b.qkv = plain_lin(arena_, v, p + "attn.qkv", true, 3 * Hv, Hv, s);
-    b.proj = plain_lin(arena_, v, p + "attn.proj", true, Hv, Hv, s);
+    b.o = plain_lin(arena_, v, p + "attn.proj", true, Hv, Hv, s);
     b.gateup = gateup_lin(arena_, v, p + "mlp.", true, d.v_inter, v_inter_pad_, Hv, s);
     b.down = plain_lin(arena_, v, p + "mlp.down_proj", true, Hv, d.v_inter, s);
     N1_CHECK(b.down.K == v_inter_pad_, "vision down_proj K padding");
@@ -199,7 +194,7 @@ void S2Model::load(const WeightSource& ws, const S2Dims& d, cudaStream_t s) {
   lblk_.resize(d.layers);
   for (int i = 0; i < d.layers; ++i) {
     const std::string p = "layers." + std::to_string(i) + ".";
-    LBlock& b = lblk_[i];
+    Block& b = lblk_[i];
     b.n1 = m.f32(arena_, p + "input_layernorm.weight", s);
     b.n2 = m.f32(arena_, p + "post_attention_layernorm.weight", s);
     b.qkv = stack_lin(arena_, m, {p + "self_attn.q_proj", p + "self_attn.k_proj", p + "self_attn.v_proj"}, true, H, s);
@@ -311,6 +306,27 @@ LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, 
   return p.release();
 }
 
+// ------------------------------------------------------------------------------------------------ transformer block
+void S2Model::block_in(const Block& b, const bf16* x, bf16* ln, bf16* qkv, const float2* rope, int rows, int H,
+                       int rot_heads, int hd, float eps, cudaStream_t s) {
+  layernorm(x, H, ln, H, b.n1, nullptr, rows, H, eps, 1, s);
+  linear(b.qkv, ln, H, qkv, b.qkv.N, rows, GemmEpilogue(), s);
+  apply_rope(qkv, b.qkv.N, rope, rows, rot_heads, hd, s);  // q and k are adjacent column blocks
+}
+
+void S2Model::block_out(const Block& b, const bf16* att, bf16* x, bf16* ln, bf16* hid, int rows, int H, int inter_pad,
+                        float eps, cudaStream_t s, bf16* save_mid) {
+  GemmEpilogue res;
+  res.residual = x, res.ldr = H;
+  linear(b.o, att, H, x, H, rows, res, s);
+  if (save_mid) N1_CUDA(cudaMemcpyAsync(save_mid, x, (size_t)rows * H * sizeof(bf16), cudaMemcpyDeviceToDevice, s));
+  layernorm(x, H, ln, H, b.n2, nullptr, rows, H, eps, 1, s);
+  GemmEpilogue sw;
+  sw.act = ACT_SWIGLU;
+  linear(b.gateup, ln, H, hid, inter_pad, rows, sw, s);
+  linear(b.down, hid, inter_pad, x, H, rows, res, s);
+}
+
 // ------------------------------------------------------------------------------------------------ vision tower
 size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s,
                          const int32_t* dst_rows_host) const {
@@ -331,10 +347,7 @@ size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* o
   gather_rows(pixels, p.window_index, xin, N, unit, patch_k_, s);  // hidden_states[window_index] on merge groups
   linear(v_patch_, xin, patch_k_, x, Hv, (int)N, GemmEpilogue(), s);
   for (int l = 0; l < dims.v_depth; ++l) {
-    const VBlock& b = vblk_[l];
-    layernorm(x, Hv, ln, Hv, b.n1, nullptr, (int)N, Hv, 1e-6f, 1, s);
-    linear(b.qkv, ln, Hv, qkv, 3 * Hv, (int)N, GemmEpilogue(), s);
-    apply_rope(qkv, 3 * Hv, p.rope, N, 2 * dims.v_heads, 80, s);  // q and k are adjacent column blocks
+    block_in(vblk_[l], x, ln, qkv, p.rope, (int)N, Hv, 2 * dims.v_heads, 80, 1e-6f, s);
     bool full = false;
     for (int i = 0; i < dims.n_fullatt; ++i) full |= dims.fullatt[i] == l;
     AttnParams a = {};
@@ -346,14 +359,7 @@ size_t S2Model::vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* o
     a.max_seq_q = full ? p.host.max_full : p.host.max_window;
     a.kv_div = 1, a.scale = 1.0f / sqrtf(80.f);
     attention(a, s);
-    GemmEpilogue res;
-    res.residual = x, res.ldr = Hv;
-    linear(b.proj, att, Hv, x, Hv, (int)N, res, s);
-    layernorm(x, Hv, ln, Hv, b.n2, nullptr, (int)N, Hv, 1e-6f, 1, s);
-    GemmEpilogue sw;
-    sw.act = ACT_SWIGLU;
-    linear(b.gateup, ln, Hv, hid, v_inter_pad_, (int)N, sw, s);
-    linear(b.down, hid, v_inter_pad_, x, Hv, (int)N, res, s);
+    block_out(vblk_[l], att, x, ln, hid, (int)N, Hv, v_inter_pad_, 1e-6f, s);
   }
   // merger: RMSNorm over Hv, then groups of merge^2 patches concatenated (a pure view), MLP with exact GELU
   layernorm(x, Hv, ln, Hv, merger_ln_, nullptr, (int)N, Hv, 1e-6f, 1, s);
@@ -393,10 +399,8 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
     N1_CUDA(cudaMemcpyAsync(image_rows, image_rows_host, p.n_image_tokens * sizeof(int), cudaMemcpyHostToDevice, s));
   build_embeds(p.kind, p.src, embed_, image_feats, latentq_, x, T, H, s, image_rows_host ? image_rows : nullptr);
   for (int l = 0; l < dims.layers; ++l) {
-    const LBlock& b = lblk_[l];
-    layernorm(x, H, ln, H, b.n1, nullptr, (int)T, H, dims.rms_eps, 1, s);
-    linear(b.qkv, ln, H, qkv, qkv_n, (int)T, GemmEpilogue(), s);
-    apply_rope(qkv, qkv_n, p.rope, T, dims.heads + dims.kv_heads, hd, s);
+    const Block& b = lblk_[l];
+    block_in(b, x, ln, qkv, p.rope, (int)T, H, dims.heads + dims.kv_heads, hd, dims.rms_eps, s);
     if (kv)  // keep the rotated keys and the values of every prompt token for the decode passes
       kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, dims.kv_heads * hd, p.dest_rows, T,
                 kv->k + l * kv->layer_stride, kv->v + l * kv->layer_stride, s);
@@ -419,8 +423,6 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
       a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
       attention(a, s);
     }
-    GemmEpilogue res;
-    res.residual = x, res.ldr = H;
     if (l == dims.layers - 1) {
       // Only the n_query TRAJ rows of each sequence are read after the last layer (internvla_n1.py L345): every token
       // still contributes K/V to the attention above, but o_proj and the MLP run on those B * n_query rows alone.
@@ -431,24 +433,12 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
       bf16* ln_sel = ln + 2L * R * H;          // [R, H]
       gather_rows(att, p.out_rows, att_sel, R, 1, H, s);
       gather_rows(x, p.out_rows, x_sel, R, 1, H, s);
-      GemmEpilogue rs;
-      rs.residual = x_sel, rs.ldr = H;
-      linear(b.o, att_sel, H, x_sel, H, R, rs, s);
-      layernorm(x_sel, H, ln_sel, H, b.n2, nullptr, R, H, dims.rms_eps, 1, s);
-      GemmEpilogue sw;
-      sw.act = ACT_SWIGLU;
-      linear(b.gateup, ln_sel, H, hid, inter_pad_, R, sw, s);
-      linear(b.down, hid, inter_pad_, x_sel, H, R, rs, s);
+      block_out(b, att_sel, x_sel, ln_sel, hid, R, H, inter_pad_, dims.rms_eps, s);
       // outputs.hidden_states[-1][:, -N_QUERY:, :] -- the last entry is post final-norm
       layernorm(x_sel, H, out, H, final_norm_, nullptr, R, H, dims.rms_eps, 1, s);
       break;
     }
-    linear(b.o, att, H, x, H, (int)T, res, s);
-    layernorm(x, H, ln, H, b.n2, nullptr, (int)T, H, dims.rms_eps, 1, s);
-    GemmEpilogue sw;
-    sw.act = ACT_SWIGLU;
-    linear(b.gateup, ln, H, hid, inter_pad_, (int)T, sw, s);
-    linear(b.down, hid, inter_pad_, x, H, (int)T, res, s);
+    block_out(b, att, x, ln, hid, (int)T, H, inter_pad_, dims.rms_eps, s);
   }
   return c.used();
 }
@@ -466,48 +456,41 @@ void S2Model::llm_prefill(const LlmPlan& p, void* ws, size_t ws_bytes, const bf1
 }
 
 // ------------------------------------------------------------------------------------------------ greedy decode
-struct S2Model::GenBufs {
-  int *cur_tok, *gen, *finished, *next, *k_len, *n_active, *out_tokens, *dest, *pos3, *kind, *src;
-  float2* rope;
-  bf16 *x, *ln, *qkv, *att, *hid, *normed, *logits;
-};
-
-namespace {
-void linear_rows(const Lin& L, const bf16* A, int lda, bf16* out, int ldo, int M, GemmEpilogue e, cudaStream_t s) {
-  e.bias = L.b;
-  gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, e, s);
+AttnParams S2Model::cache_attn(const LlmPlan& p, int per_seq, const int* k_len, const bf16* qkv, const bf16* k,
+                               const bf16* v, bf16* o) const {
+  const int hd = dims.head_dim;
+  AttnParams a = {};
+  a.q = qkv, a.k = k, a.v = v, a.o = o;
+  a.ldq = (dims.heads + 2 * dims.kv_heads) * hd, a.ldk = a.ldv = dims.kv_heads * hd, a.ldo = dims.hidden;
+  a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
+  a.batch = p.B, a.seq_q = per_seq, a.k_len = k_len, a.k_slot = p.slot, a.k_row0 = p.row0;
+  a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
+  return a;
 }
-}  // namespace
 
 // One pass of B * per_seq new tokens (rows of g.x) through all layers against the cache: per_seq = 1 is a decode step,
-// per_seq = 1 + n_query the latent pass.  g.dest / g.rope / g.k_len describe the chunk (gen_rows).  Result: final-norm
-// states of every row in g.normed.
-void S2Model::chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, int per_seq, cudaStream_t s) const {
+// per_seq = 1 + n_query the latent pass, per_seq = n_query the training forward.  g.dest / g.rope / g.k_len describe the
+// chunk (gen_rows).  Result: final-norm states of every row in g.normed, the last residual stream in g.x.  With `save`
+// each layer's input, q|k|v, attention output and post-attention residual go to its per-layer arrays, and g.qkv / g.att
+// are not used.
+void S2Model::chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, int per_seq, cudaStream_t s,
+                         const ChunkSaves* save) const {
   const int H = dims.hidden, hd = dims.head_dim, R = p.B * per_seq;
   const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd, kvd = dims.kv_heads * hd;
   for (int l = 0; l < dims.layers; ++l) {
-    const LBlock& b = lblk_[l];
-    layernorm(g.x, H, g.ln, H, b.n1, nullptr, R, H, dims.rms_eps, 1, s);
-    linear_rows(b.qkv, g.ln, H, g.qkv, qkv_n, R, GemmEpilogue(), s);
-    apply_rope(g.qkv, qkv_n, g.rope, R, dims.heads + dims.kv_heads, hd, s);
+    const Block& b = lblk_[l];
+    bf16* qkv = save ? save->qkv + (size_t)l * R * qkv_n : g.qkv;
+    bf16* att = save ? save->att + (size_t)l * R * H : g.att;
+    if (save)
+      N1_CUDA(cudaMemcpyAsync(save->x_in + (size_t)l * R * H, g.x, (size_t)R * H * sizeof(bf16), cudaMemcpyDeviceToDevice,
+                              s));
+    block_in(b, g.x, g.ln, qkv, g.rope, R, H, dims.heads + dims.kv_heads, hd, dims.rms_eps, s);
     bf16* ck = kv.k + l * kv.layer_stride;
     bf16* cv = kv.v + l * kv.layer_stride;
-    kv_append(g.qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, kvd, g.dest, R, ck, cv, s);
-    AttnParams a = {};
-    a.q = g.qkv, a.k = ck, a.v = cv, a.o = g.att;
-    a.ldq = qkv_n, a.ldk = a.ldv = kvd, a.ldo = H;
-    a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
-    a.batch = p.B, a.seq_q = per_seq, a.k_len = g.k_len, a.k_slot = p.slot, a.k_row0 = p.row0;
-    a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
-    attention(a, s);
-    GemmEpilogue res;
-    res.residual = g.x, res.ldr = H;
-    linear_rows(b.o, g.att, H, g.x, H, R, res, s);
-    layernorm(g.x, H, g.ln, H, b.n2, nullptr, R, H, dims.rms_eps, 1, s);
-    GemmEpilogue sw;
-    sw.act = ACT_SWIGLU;
-    linear_rows(b.gateup, g.ln, H, g.hid, inter_pad_, R, sw, s);
-    linear_rows(b.down, g.hid, inter_pad_, g.x, H, R, res, s);
+    kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, kvd, g.dest, R, ck, cv, s);
+    attention(cache_attn(p, per_seq, g.k_len, qkv, ck, cv, att), s);
+    block_out(b, att, g.x, g.ln, g.hid, R, H, inter_pad_, dims.rms_eps, s,
+              save ? save->x_mid + (size_t)l * R * H : nullptr);
   }
   layernorm(g.x, H, g.normed, H, final_norm_, nullptr, R, H, dims.rms_eps, 1, s);
 }
@@ -545,7 +528,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   int steps = 0;
   for (int it = 0; it < p.max_new; ++it) {
     // logits = lm_head(hidden[:, -1]) in bf16, next = argmax (GenerationMixin greedy search)
-    linear_rows(lm_head_, g.normed, H, g.logits, dims.vocab, B, GemmEpilogue(), s);
+    linear(lm_head_, g.normed, H, g.logits, dims.vocab, B, GemmEpilogue(), s);
     argmax_rows(g.logits, dims.vocab, dims.vocab, B, g.next, s);
     gen_update(g.next, g.cur_tok, g.gen, g.finished, g.out_tokens, p.max_new, eos, n_eos, B, g.n_active, s);
     int active = 0;

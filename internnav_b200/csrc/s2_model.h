@@ -129,6 +129,8 @@ class S2Model {
   // workspace: the forward leaves the cache and the per-layer TRAJ-row tensors there for the backward.
   // overwrite the library's copy of `latent_queries` (bf16 [n_query, hidden], device) after an optimizer step
   void set_latent_queries(const bf16* src, cudaStream_t s);
+  // Refuses a continuation plan (one created over a K/V pool: its rows live in the pool, not in the workspace's cache).
+  // train_forward and train_backward size their workspace here before they launch anything, so they refuse it too.
   size_t ws_train(const LlmPlan& p) const;
   // -> states bf16 [B, n_query, hidden] = hidden_states[b, t_s_pos[b] : t_s_pos[b] + n_query] (internvla_n1.py L231-235)
   void train_forward(const LlmPlan& p, void* ws, size_t ws_bytes, const bf16* image_feats, bf16* states, cudaStream_t s);
@@ -141,40 +143,55 @@ class S2Model {
     bf16 *k = nullptr, *v = nullptr;  // [layers][B * slot][kv_heads * head_dim]
     long layer_stride = 0;
   };
-  struct GenBufs;
-  struct VBlock {
-    float *n1 = nullptr, *n2 = nullptr;
-    Lin qkv, proj, gateup, down;
+  // decode-state buffers of gen_impl; the training forward carves the chunk's share of them (s2_train.cu)
+  struct GenBufs {
+    int *cur_tok = nullptr, *gen = nullptr, *finished = nullptr, *next = nullptr, *k_len = nullptr, *n_active = nullptr;
+    int *out_tokens = nullptr, *dest = nullptr, *pos3 = nullptr, *kind = nullptr, *src = nullptr;
+    float2* rope = nullptr;
+    bf16 *x = nullptr, *ln = nullptr, *qkv = nullptr, *att = nullptr, *hid = nullptr, *normed = nullptr, *logits = nullptr;
   };
-  struct LBlock {
+  // per-layer tensors of a chunk pass that the training backward reads: layer l's R rows start at row l * R
+  struct ChunkSaves {
+    bf16 *x_in = nullptr, *qkv = nullptr, *att = nullptr, *x_mid = nullptr;  // layer input, q|k|v, attention, post-attention
+  };
+  // weights of one pre-norm block, vision tower and decoder alike
+  struct Block {
     float *n1 = nullptr, *n2 = nullptr;
     Lin qkv, o, gateup, down;
   };
+  // One pre-norm block, split around the step that differs per pass (K/V append and attention); x [rows, H] is the
+  // residual stream.  block_in: ln = RMSNorm(x); qkv = linear(ln); RoPE on its first rot_heads heads (q and k).
+  static void block_in(const Block& b, const bf16* x, bf16* ln, bf16* qkv, const float2* rope, int rows, int H,
+                       int rot_heads, int hd, float eps, cudaStream_t s);
+  // block_out: x += linear(att); save_mid (if set) = x; x += down(SwiGLU(gateup(RMSNorm(x)))), hid [rows, inter_pad]
+  static void block_out(const Block& b, const bf16* att, bf16* x, bf16* ln, bf16* hid, int rows, int H, int inter_pad,
+                        float eps, cudaStream_t s, bf16* save_mid = nullptr);
+  // causal attention of per_seq new rows per sequence (packed q|k|v rows) on one layer's slotted K/V cache
+  AttnParams cache_attn(const LlmPlan& p, int per_seq, const int* k_len, const bf16* qkv, const bf16* k, const bf16* v,
+                        bf16* o) const;
   size_t vit_impl(Carver c, const VitPlan& p, const bf16* pixels, bf16* out, cudaStream_t s,
                   const int32_t* dst_rows_host = nullptr) const;
   size_t llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf16* out, cudaStream_t s,
                   const KvCache* kv = nullptr, const int32_t* image_rows_host = nullptr) const;
   size_t gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, const int32_t* eos, int n_eos, int32_t pad,
                   GenResult* out, bf16* latents, cudaStream_t s, const int32_t* image_rows_host = nullptr) const;
-  void chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, int per_seq, cudaStream_t s) const;
+  void chunk_pass(const GenBufs& g, const LlmPlan& p, const KvCache& kv, int per_seq, cudaStream_t s,
+                  const ChunkSaves* save = nullptr) const;
 
   Arena arena_;
   bool loaded_ = false;
   int v_inter_pad_ = 0, inter_pad_ = 0, patch_k_ = 0;
   Lin v_patch_;
-  std::vector<VBlock> vblk_;
+  std::vector<Block> vblk_;
   float* merger_ln_ = nullptr;
   Lin merger0_, merger2_;
   bf16* embed_ = nullptr;    // [vocab, hidden]
   bf16* latentq_ = nullptr;  // [n_query, hidden]; null for a System-2-only checkpoint
-  std::vector<LBlock> lblk_;
+  std::vector<Block> lblk_;
   float* final_norm_ = nullptr;
   Lin lm_head_;  // optional ("lm_head.weight"); only generate() needs it
-  // transposed copies of the frozen decoder weights for the dgrad GEMMs of train_backward (built on first use)
-  struct LBlockT {
-    Lin qkv, o, gateup, down;
-  };
-  std::vector<LBlockT> lblk_t_;
+  // transposed copies of the frozen decoder weights for the dgrad GEMMs of train_backward (built on first use; no norms)
+  std::vector<Block> lblk_t_;
   struct TrainBufs;
   size_t train_carve(Carver& c, const LlmPlan& p, TrainBufs& t) const;
   void ensure_transposed(cudaStream_t s);

@@ -1,7 +1,5 @@
 // Training branch, System-2 half: TRAJ-row forward on the prompt's K/V cache and its backward to latent_queries.
 // Algorithm and parity target: oracle/qwen_backward.py (equal to autograd through the padded-batch forward).
-#include <math.h>
-
 #include <algorithm>
 
 #include "bwd_kernels.h"
@@ -42,10 +40,6 @@ __global__ void sum_over_batch_kernel(const bf16* __restrict__ d, int B, int nq,
   out[i] = acc;
 }
 
-void linear_t(const Lin& L, const bf16* A, int lda, bf16* out, int ldo, int M, cudaStream_t s) {
-  gemm_bf16(A, lda, L.w, L.ldw, out, ldo, M, L.N, L.K, GemmEpilogue(), s);
-}
-
 Lin transposed(Arena& a, const Lin& L, cudaStream_t s) {
   Lin T;
   T.N = L.K, T.K = (L.N + 7) & ~7, T.ldw = T.K;  // out = A @ T.w^T with T.w [K_orig, N_orig]: dX = dY @ W
@@ -58,10 +52,8 @@ Lin transposed(Arena& a, const Lin& L, cudaStream_t s) {
 
 struct S2Model::TrainBufs {
   KvCache kv;
-  int *gen, *k_len, *dest, *pos3, *kind, *src;
-  float2* rope;
-  bf16 *x_in, *qkv, *att, *x_mid, *x_final;        // per-layer saves: [layers][R, .] (x_final: [R, H])
-  bf16 *x, *ln, *hid;                                // forward scratch
+  GenBufs g;        // the TRAJ chunk: its row description and forward scratch; g.x ends as the last residual stream
+  ChunkSaves save;  // per-layer saves: [layers][R, .]
   bf16 *d, *pre, *dpre, *dact, *da, *dqkv, *dh;     // backward scratch
   float *dk, *dv;                                    // [B * slot, kvd] fp32
   int R;
@@ -87,12 +79,13 @@ size_t S2Model::train_carve(Carver& c, const LlmPlan& p, TrainBufs& t) const {
   t.kv.layer_stride = (long)B * p.slot * kvd;
   t.kv.k = c.take<bf16>((size_t)L * t.kv.layer_stride);
   t.kv.v = c.take<bf16>((size_t)L * t.kv.layer_stride);
-  t.gen = c.take<int>(B), t.k_len = c.take<int>(B), t.dest = c.take<int>(R), t.pos3 = c.take<int>(3 * R);
-  t.kind = c.take<int>(R), t.src = c.take<int>(R);
-  t.rope = c.take<float2>((size_t)R * (hd / 2));
-  t.x_in = c.take<bf16>((size_t)L * R * H), t.qkv = c.take<bf16>((size_t)L * R * qkv_n);
-  t.att = c.take<bf16>((size_t)L * R * H), t.x_mid = c.take<bf16>((size_t)L * R * H), t.x_final = c.take<bf16>((size_t)R * H);
-  t.x = c.take<bf16>((size_t)R * H), t.ln = c.take<bf16>((size_t)R * H), t.hid = c.take<bf16>((size_t)R * inter_pad_);
+  GenBufs& g = t.g;
+  g.gen = c.take<int>(B), g.k_len = c.take<int>(B), g.dest = c.take<int>(R), g.pos3 = c.take<int>(3 * R);
+  g.kind = c.take<int>(R), g.src = c.take<int>(R);
+  g.rope = c.take<float2>((size_t)R * (hd / 2));
+  t.save.x_in = c.take<bf16>((size_t)L * R * H), t.save.qkv = c.take<bf16>((size_t)L * R * qkv_n);
+  t.save.att = c.take<bf16>((size_t)L * R * H), t.save.x_mid = c.take<bf16>((size_t)L * R * H);
+  g.x = c.take<bf16>((size_t)R * H), g.ln = c.take<bf16>((size_t)R * H), g.hid = c.take<bf16>((size_t)R * inter_pad_);
   t.d = c.take<bf16>((size_t)R * H), t.pre = c.take<bf16>((size_t)R * 2 * inter_pad_);
   t.dpre = c.take<bf16>((size_t)R * 2 * inter_pad_), t.dact = c.take<bf16>((size_t)R * inter_pad_);
   t.da = c.take<bf16>((size_t)R * H), t.dqkv = c.take<bf16>((size_t)R * qkv_n), t.dh = c.take<bf16>((size_t)R * H);
@@ -107,6 +100,9 @@ void S2Model::set_latent_queries(const bf16* src, cudaStream_t s) {
 }
 
 size_t S2Model::ws_train(const LlmPlan& p) const {
+  // a continuation plan's dest_rows index pool rows (slot * pool_cap + ...), which lie outside the B * slot rows per
+  // layer of the workspace's cache
+  N1_CHECK(!p.pool, "training: the plan continues a K/V pool; training needs a generation plan created without a pool");
   N1_CHECK(p.max_new > 0, "ws_train: needs a generation plan (prompts without TRAJ tokens)");
   Carver c(nullptr, 0);
   TrainBufs t;
@@ -122,53 +118,22 @@ void S2Model::train_forward(const LlmPlan& p, void* ws, size_t ws_bytes, const b
   if (ws_bytes < ws_train(p)) throw Error(-7, "train_forward: workspace too small");
   p.wait_ready(s);
   const int H = dims.hidden, hd = dims.head_dim, nq = dims.n_query;
-  const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd, kvd = dims.kv_heads * hd;
   Carver c(ws, ws_bytes);
   TrainBufs t;
   train_carve(c, p, t);
+  GenBufs& g = t.g;
   const int R = t.R;
   // 1. prompt prefill with the K/V of every layer kept (the value it returns -- last prompt row -- is not needed)
-  llm_impl(c, p, image_feats, t.ln, s, &t.kv);
+  llm_impl(c, p, image_feats, g.ln, s, &t.kv);
   // 2. the n_query TRAJ rows of every sample as one chunk on that cache: rows len .. len + n_query - 1
-  N1_CUDA(cudaMemsetAsync(t.gen, 0, p.B * sizeof(int), s));
-  gen_rows(p.d_len, p.d_delta, t.gen, 0, nq, p.B, p.slot, nullptr, t.dest, t.pos3, t.k_len, s);
-  mrope_table(t.pos3, t.rope, R, hd / 2, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
-  fill_latent_rows_kernel<<<nblk(R), 256, 0, s>>>(t.kind, t.src, R, nq);
+  N1_CUDA(cudaMemsetAsync(g.gen, 0, p.B * sizeof(int), s));
+  gen_rows(p.d_len, p.d_delta, g.gen, 0, nq, p.B, p.slot, nullptr, g.dest, g.pos3, g.k_len, s);
+  mrope_table(g.pos3, g.rope, R, hd / 2, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
+  fill_latent_rows_kernel<<<nblk(R), 256, 0, s>>>(g.kind, g.src, R, nq);
   N1_CUDA(cudaGetLastError());
-  build_embeds(t.kind, t.src, embed_, nullptr, latentq_, t.x, R, H, s);
-  const size_t row_bytes = (size_t)R * H * sizeof(bf16);
-  for (int l = 0; l < dims.layers; ++l) {
-    const LBlock& b = lblk_[l];
-    bf16* qkv = t.qkv + (size_t)l * R * qkv_n;
-    bf16* att = t.att + (size_t)l * R * H;
-    N1_CUDA(cudaMemcpyAsync(t.x_in + (size_t)l * R * H, t.x, row_bytes, cudaMemcpyDeviceToDevice, s));
-    layernorm(t.x, H, t.ln, H, b.n1, nullptr, R, H, dims.rms_eps, 1, s);
-    GemmEpilogue e;
-    e.bias = b.qkv.b;
-    gemm_bf16(t.ln, H, b.qkv.w, b.qkv.ldw, qkv, qkv_n, R, b.qkv.N, b.qkv.K, e, s);
-    apply_rope(qkv, qkv_n, t.rope, R, dims.heads + dims.kv_heads, hd, s);
-    bf16* ck = t.kv.k + l * t.kv.layer_stride;
-    bf16* cv = t.kv.v + l * t.kv.layer_stride;
-    kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, kvd, t.dest, R, ck, cv, s);
-    AttnParams a = {};
-    a.q = qkv, a.k = ck, a.v = cv, a.o = att;
-    a.ldq = qkv_n, a.ldk = a.ldv = kvd, a.ldo = H;
-    a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
-    a.batch = p.B, a.seq_q = nq, a.k_len = t.k_len, a.k_slot = p.slot;
-    a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
-    attention(a, s);
-    GemmEpilogue res;
-    res.residual = t.x, res.ldr = H;
-    gemm_bf16(att, H, b.o.w, b.o.ldw, t.x, H, R, b.o.N, b.o.K, res, s);
-    N1_CUDA(cudaMemcpyAsync(t.x_mid + (size_t)l * R * H, t.x, row_bytes, cudaMemcpyDeviceToDevice, s));
-    layernorm(t.x, H, t.ln, H, b.n2, nullptr, R, H, dims.rms_eps, 1, s);
-    GemmEpilogue sw;
-    sw.act = ACT_SWIGLU;
-    gemm_bf16(t.ln, H, b.gateup.w, b.gateup.ldw, t.hid, inter_pad_, R, b.gateup.N, b.gateup.K, sw, s);
-    gemm_bf16(t.hid, inter_pad_, b.down.w, b.down.ldw, t.x, H, R, b.down.N, b.down.K, res, s);
-  }
-  N1_CUDA(cudaMemcpyAsync(t.x_final, t.x, row_bytes, cudaMemcpyDeviceToDevice, s));
-  layernorm(t.x, H, states, H, final_norm_, nullptr, R, H, dims.rms_eps, 1, s);
+  build_embeds(g.kind, g.src, embed_, nullptr, latentq_, g.x, R, H, s);
+  g.normed = states;
+  chunk_pass(g, p, t.kv, nq, s, &t.save);
   p.mark_used(s);
 }
 
@@ -186,39 +151,34 @@ void S2Model::train_backward(const LlmPlan& p, void* ws, size_t ws_bytes, const 
   train_carve(c, p, t);
   const int R = t.R;
   const float eps = dims.rms_eps;
-  norm_bwd(grad_states, H, t.x_final, H, final_norm_, nullptr, 0, t.d, H, nullptr, nullptr, R, H, eps, 1, 0, s);
+  const GenBufs& g = t.g;
+  norm_bwd(grad_states, H, g.x, H, final_norm_, nullptr, 0, t.d, H, nullptr, nullptr, R, H, eps, 1, 0, s);
   for (int l = dims.layers - 1; l >= 0; --l) {
-    const LBlock& b = lblk_[l];
-    const LBlockT& bt = lblk_t_[l];
-    const bf16* x_in = t.x_in + (size_t)l * R * H;
-    const bf16* x_mid = t.x_mid + (size_t)l * R * H;
-    const bf16* qkv = t.qkv + (size_t)l * R * qkv_n;
-    const bf16* att = t.att + (size_t)l * R * H;
+    const Block& b = lblk_[l];
+    const Block& bt = lblk_t_[l];
+    const bf16* x_in = t.save.x_in + (size_t)l * R * H;
+    const bf16* x_mid = t.save.x_mid + (size_t)l * R * H;
     // MLP: recompute the gate / up pre-activations of these rows, then dgrad through down, SwiGLU, gate/up
-    layernorm(x_mid, H, t.ln, H, b.n2, nullptr, R, H, eps, 1, s);
-    gemm_bf16(t.ln, H, b.gateup.w, b.gateup.ldw, t.pre, 2 * inter_pad_, R, b.gateup.N, b.gateup.K, GemmEpilogue(), s);
-    linear_t(bt.down, t.d, H, t.dact, inter_pad_, R, s);
+    layernorm(x_mid, H, g.ln, H, b.n2, nullptr, R, H, eps, 1, s);
+    linear(b.gateup, g.ln, H, t.pre, 2 * inter_pad_, R, GemmEpilogue(), s);
+    linear(bt.down, t.d, H, t.dact, inter_pad_, R, GemmEpilogue(), s);
     swiglu_bwd(t.pre, t.dact, t.dpre, R, inter_pad_, s);
-    linear_t(bt.gateup, t.dpre, 2 * inter_pad_, t.dh, H, R, s);
+    linear(bt.gateup, t.dpre, 2 * inter_pad_, t.dh, H, R, GemmEpilogue(), s);
     norm_bwd(t.dh, H, x_mid, H, b.n2, t.d, H, t.d, H, nullptr, nullptr, R, H, eps, 1, 0, s);
     // attention: dO = d W_o ; backward of n_query queries per sample over the visible keys of the cache
-    linear_t(bt.o, t.d, H, t.da, H, R, s);
+    linear(bt.o, t.d, H, t.da, H, R, GemmEpilogue(), s);
     N1_CUDA(cudaMemsetAsync(t.dk, 0, (size_t)p.B * p.slot * kvd * sizeof(float), s));
     N1_CUDA(cudaMemsetAsync(t.dv, 0, (size_t)p.B * p.slot * kvd * sizeof(float), s));
     AttnBwdParams ab = {};
-    ab.f.q = qkv, ab.f.k = t.kv.k + l * t.kv.layer_stride, ab.f.v = t.kv.v + l * t.kv.layer_stride;
-    ab.f.o = const_cast<bf16*>(att);
-    ab.f.ldq = qkv_n, ab.f.ldk = ab.f.ldv = kvd, ab.f.ldo = H;
-    ab.f.heads_q = dims.heads, ab.f.heads_kv = dims.kv_heads, ab.f.hd = hd;
-    ab.f.batch = p.B, ab.f.seq_q = nq, ab.f.k_len = t.k_len, ab.f.k_slot = p.slot;
-    ab.f.kv_div = 1, ab.f.causal = 1, ab.f.scale = 1.0f / sqrtf((float)hd);
+    ab.f = cache_attn(p, nq, g.k_len, t.save.qkv + (size_t)l * R * qkv_n, t.kv.k + l * t.kv.layer_stride,
+                      t.kv.v + l * t.kv.layer_stride, t.save.att + (size_t)l * R * H);
     ab.dout = t.da, ab.lddo = H, ab.dq = t.dqkv, ab.lddq = qkv_n, ab.dk = t.dk, ab.dv = t.dv;
     attention_bwd(ab, s);
-    gather_kv_grad_kernel<<<nblk((long)R * kvd), 256, 0, s>>>(t.dk, t.dv, t.dest, R, kvd, t.dqkv, qkv_n, dims.heads * hd,
+    gather_kv_grad_kernel<<<nblk((long)R * kvd), 256, 0, s>>>(t.dk, t.dv, g.dest, R, kvd, t.dqkv, qkv_n, dims.heads * hd,
                                                             (dims.heads + dims.kv_heads) * hd);
     N1_CUDA(cudaGetLastError());
-    rope_transposed(t.dqkv, qkv_n, t.rope, R, dims.heads + dims.kv_heads, hd, s);
-    linear_t(bt.qkv, t.dqkv, qkv_n, t.dh, H, R, s);
+    rope_transposed(t.dqkv, qkv_n, g.rope, R, dims.heads + dims.kv_heads, hd, s);
+    linear(bt.qkv, t.dqkv, qkv_n, t.dh, H, R, GemmEpilogue(), s);
     norm_bwd(t.dh, H, x_in, H, b.n1, t.d, H, t.d, H, nullptr, nullptr, R, H, eps, 1, 0, s);
   }
   sum_over_batch_kernel<<<nblk((long)nq * H), 256, 0, s>>>(t.d, p.B, nq, H, grad_latent);
