@@ -21,9 +21,10 @@ import numpy as np
 import torch
 from PIL import Image
 
+from .preprocess import SYS1_DEPTH_THRESHOLD   # internvla_n1_agent.py L60
+
 LOOK_DOWN = 5
 SYS1_FORWARD_STEP = 4        # internvla_n1_agent.py L61
-SYS1_DEPTH_THRESHOLD = 5.0   # L60
 
 
 class PerEnvPolicies:
@@ -57,7 +58,8 @@ class PerEnvPolicies:
 
 
 def intrinsic_matrix(width, height, hfov):
-    """internvla_n1_agent.py L119-131."""
+    """Pinhole intrinsics [4, 4] of a width x height sensor with horizontal field of view `hfov` degrees (square
+    pixels, principal point at the centre of the pixel grid): internvla_n1_agent.py L119-131."""
     fx = (width / 2.0) / np.tan(np.deg2rad(hfov / 2.0))
     return np.array([[fx, 0.0, (width - 1.0) / 2.0, 0.0], [0.0, fx, (height - 1.0) / 2.0, 0.0],
                      [0.0, 0.0, 1.0, 0.0], [0.0, 0.0, 0.0, 1.0]])

@@ -19,12 +19,11 @@ System 2 -- prompts, image history, look-down turns, the device image path, the 
 `InternVLAN1Policy`.  A step makes one System-2 call for every robot that is due, `serve` at most one more for the robots
 that answered [5], and then one `generate_traj` call covers every robot that holds a latent plan.
 
-On a CUDA device the System-1 frames are prepared on the GPU: the current frames of all robots that need System 1 are
-resized in one `FramePreprocessor` call, and each robot keeps its pixel-goal frame on the device, already resized (the
-reference resizes the same bytes again on every step, with the same result).  Depth is resized (no scaling, no clip)
-only for a System 1 that reads it (`navdp_async`); `nextdit_async` does not.  The reference hands System 1 float64
-frames; this library's System 1 takes float32, which holds x / 255 of every byte exactly as the reference's
-`generate_traj` consumes it after its own conversion.  On the CPU the frames are resized with Pillow, as in the reference.
+The System-1 frames, the pixel-goal frames and the `generate_traj` call are `preprocess.System1Inputs`: on a CUDA device
+the current frames of all robots that need System 1 are resized in one `FramePreprocessor` call, on the CPU with Pillow,
+as in the reference.  Depth is resized (no scaling, no clip) only for a System 1 that reads it (`navdp_async`);
+`nextdit_async` does not.  The reference hands System 1 float64 frames; this library's System 1 takes float32, which
+holds x / 255 of every byte exactly as the reference's `generate_traj` consumes it after its own conversion.
 
 Deviations from the reference class:
   * nothing is written to `save_dir` (no debug images, no answer files) and nothing is printed;
@@ -36,12 +35,11 @@ Deviations from the reference class:
 """
 import numpy as np
 import torch
-from PIL import Image
 
 from . import policy as P
 from .postprocess import batched_traj_to_waypoints
+from .preprocess import FramePreprocessor, System1Inputs
 
-S1_SIZE = 224
 LOOK_DOWN = [5]
 
 
@@ -56,13 +54,13 @@ class S2Output(P.S2Output):
 
 
 class _Robot:
-    """What System 2 last told one robot (the reference's output_action / output_latent / output_pixel, last_s2_idx and
-    the pixel-goal frame, resized to 224 x 224)."""
-    __slots__ = ("last_s2_idx", "action", "latent", "pixel", "goal_rgb", "goal_depth")
+    """What System 2 last told one robot (the reference's output_action / output_latent / output_pixel and
+    last_s2_idx)."""
+    __slots__ = ("last_s2_idx", "action", "latent", "pixel")
 
     def __init__(self):
         self.last_s2_idx = -100
-        self.action = self.latent = self.pixel = self.goal_rgb = self.goal_depth = None
+        self.action = self.latent = self.pixel = None
 
 
 class InternVLAN1AsyncAgent:
@@ -86,16 +84,14 @@ class InternVLAN1AsyncAgent:
             raise ValueError("InternVLAN1AsyncAgent needs a model with a System 1 (the DualVLN checkpoint); this one has "
                              "none: serve it with InternVLAN1Policy")
         self.model, self.processor = model, processor
-        self.num_envs, self.x_init = int(num_envs), x_init
+        self.num_envs = int(num_envs)
         self.plan_step_gap = np.broadcast_to(np.asarray(args.plan_step_gap, dtype=np.int64), (self.num_envs,))
         self.policy = P.InternVLAN1Policy(model, processor, num_envs=num_envs, num_history=args.num_history,
                                           resize_w=args.resize_w, resize_h=args.resize_h, device=self.device,
                                           vision_cache_frames=vision_cache_frames)
         self.reads_depth = getattr(getattr(model, "config", None), "system1", None) == "navdp_async"
-        self._frames = None
-        if self.device.type == "cuda":
-            from .preprocess import FramePreprocessor
-            self._frames = FramePreprocessor(self.device, out_size=S1_SIZE)
+        self._frames = FramePreprocessor(self.device) if self.device.type == "cuda" else None
+        self.s1 = System1Inputs(model, self._frames, x_init)
         self.robots = [_Robot() for _ in range(num_envs)]
         self.calls = {"s2": 0, "s1": 0}
 
@@ -104,6 +100,7 @@ class InternVLAN1AsyncAgent:
         for e in envs:
             self.robots[e] = _Robot()
         self.policy.reset(list(envs))
+        self.s1.reset(envs)
 
     # ------------------------------------------------------------------ L127-164
     def step(self, env_ids, rgbs, depths, poses, instructions, intrinsic=None, look_downs=None):
@@ -193,49 +190,10 @@ class InternVLAN1AsyncAgent:
         if not s1:
             return
         envs = [env_ids[j] for j in s1]
-        cur = self._rgb224([rgbs[j] for j in s1])
-        cur_d = self._depth224([depths[j] for j in s1]) if self.reads_depth else None
-        for k, e in enumerate(envs):
-            if e in goals:
-                self.robots[e].goal_rgb = cur[k].clone()
-                self.robots[e].goal_depth = None if cur_d is None else cur_d[k].clone()
-        rgb = torch.stack([torch.stack((self.robots[e].goal_rgb, cur[k])) for k, e in enumerate(envs)])
-        dep = None
-        if cur_d is not None:
-            dep = torch.stack([torch.stack((self.robots[e].goal_depth, cur_d[k])) for k, e in enumerate(envs)])[..., None]
-        lat = torch.cat([self.robots[e].latent.reshape(1, *self.robots[e].latent.shape[-2:]) for e in envs])
-        kw = {} if self.x_init is None else {"x_init": self.x_init(envs)}
-        with torch.no_grad():
-            traj = self.model.generate_traj(lat, rgb, dep, **kw)
+        cur = self.s1.rgb([rgbs[j] for j in s1])
+        cur_d = self.s1.depth([depths[j] for j in s1]) if self.reads_depth else None
+        traj = self.s1.generate(envs, goals, cur, cur_d, [self.robots[e].latent for e in envs])
         self.calls["s1"] += 1
         paths = batched_traj_to_waypoints(traj, len(envs))
         for k, j in enumerate(s1):
             outs[j].output_trajectory = paths[k]
-
-    def _rgb224(self, frames):
-        """Raw uint8 frames -> float32 [n, 224, 224, 3] = Pillow-resized / 255, on the agent's device."""
-        if self._frames is None:
-            return torch.from_numpy(np.stack([np.array(Image.fromarray(np.asarray(f)).resize((S1_SIZE, S1_SIZE))) / 255.0
-                                              for f in frames])).float()
-        return self._by_shape(frames, self._frames.rgb)
-
-    def _depth224(self, frames):
-        """Raw float32 depth [H, W] -> float32 [n, 224, 224], Pillow-resized (mode F), no scaling, no clip."""
-        frames = [np.asarray(f, dtype=np.float32).reshape(np.asarray(f).shape[:2]) for f in frames]
-        if self._frames is None:
-            return torch.from_numpy(np.stack([np.array(Image.fromarray(f).resize((S1_SIZE, S1_SIZE))) for f in frames]))
-        return self._by_shape(frames, lambda x: self._frames.depth(x, mul=1.0, clip_max=float("inf")))
-
-    @staticmethod
-    def _by_shape(frames, resize):
-        """One resize call per distinct frame shape (one in all for a fleet of identical cameras)."""
-        groups = {}
-        for k, f in enumerate(frames):
-            groups.setdefault(np.asarray(f).shape, []).append(k)
-        out = [None] * len(frames)
-        for idx in groups.values():
-            r = resize(torch.from_numpy(np.stack([np.asarray(frames[k]) for k in idx])))
-            for i, k in enumerate(idx):
-                out[k] = r[i]
-        return torch.stack(out) if len(groups) > 1 else r
-

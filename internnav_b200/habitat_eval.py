@@ -23,13 +23,13 @@ every System-1 request in ONE `generate_traj` call followed by `batched_traj_to_
 environment whose episode ends resets and goes on with its next episode in the same round.
 
 System 2 -- prompts, image history, look-down turns, the device image path, the K/V and feature pools -- is
-`InternVLAN1Policy`.  On a CUDA device the System-1 RGB frames of a round are uploaded and resized in one
-`FramePreprocessor.rgb` call and cast to bf16: the kernel's float32 u / 255 rounded to bf16 is torch's
-`bf16(u8) / 255` for every byte.  Each environment keeps its pixel-goal frame on the device.  Depth is prepared only for
-a System 1 that reads it (`navdp_async`): `depth_filter` runs on the full frame on the host, as in the reference; then
-only the 224 x 224 source pixels of Pillow's NEAREST resize are taken (`nearest_index`) and the affine, `* 1000`, the
-uint16 truncation, `/ 1000`, float32, the clip at 5 and bf16 are applied to those samples.  Every step after the filter
-is element-wise, so this is the reference's full-frame path bit for bit.  On the CPU the frames go through Pillow.
+`InternVLAN1Policy`.  The System-1 RGB frames, the pixel-goal frames and the `generate_traj` call are
+`preprocess.System1Inputs`: the RGB frames of a round are resized in one call (`FramePreprocessor` on a CUDA device,
+Pillow on the CPU) to float32 u / 255 and cast to bf16, which is torch's `bf16(u8) / 255` for every byte.  Depth is
+prepared only for a System 1 that reads it (`navdp_async`), on the host: `depth_filter` runs on the full frame, as in
+the reference; then only the 224 x 224 source pixels of Pillow's NEAREST resize are taken (`nearest_index`) and the
+affine, `* 1000`, the uint16 truncation, `/ 1000`, float32, the clip at 5 and bf16 are applied to those samples.  Every
+step after the filter is element-wise, so this is the reference's full-frame path bit for bit.
 
 Deviations from the reference loop:
   * nothing is written (no check_sim images, videos, progress.json or resume) and nothing is printed; the caller
@@ -70,16 +70,14 @@ import random
 
 import numpy as np
 import torch
-from PIL import Image
 
 from . import policy as P
-from .agent_realworld import InternVLAN1AsyncAgent
+from .agent import intrinsic_matrix
 from .postprocess import batched_traj_to_actions
+from .preprocess import S1_SIZE, SYS1_DEPTH_THRESHOLD, FramePreprocessor, System1Inputs
 
-S1_SIZE = 224
 MAX_STEPS, MAX_LOCAL_STEPS = 8, 4
 STOP, FORWARD, LEFT, RIGHT, LOOKUP, LOOKDOWN = range(6)
-DEPTH_CLIP = 5.0
 CAMERA_PITCH = np.deg2rad(30)      # the pitch the system2 loop assumes for every pixel answer (L718)
 FOLLOWER_RADIUS = 0.25             # ShortestPathFollower(sim, 0.25, False), once per episode (L663)
 CONJUNCTIONS = ["you can see ", "in front of you is ", "there is ", "you can spot ", "you are toward the ",
@@ -137,14 +135,6 @@ def agent_to_world(state):
     return m
 
 
-def intrinsic_matrix(width, height, hfov):
-    """Pinhole intrinsics [4, 4] of a width x height sensor with horizontal field of view `hfov` degrees (square
-    pixels, principal point at the centre of the pixel grid)."""
-    f = (width / 2.0) / np.tan(np.deg2rad(hfov / 2.0))
-    return np.array([[f, 0.0, (width - 1.0) / 2.0, 0.0], [0.0, f, (height - 1.0) / 2.0, 0.0],
-                     [0.0, 0.0, 1.0, 0.0], [0.0, 0.0, 0.0, 1.0]])
-
-
 def camera_to_episodic(xyz, yaw, pitch=CAMERA_PITCH):
     """Camera -> episodic frame [4, 4]: yaw about z, then pitch about y, at position xyz, times the axis alignment that
     takes the camera's (right, down, forward) axes to (forward, left, up)."""
@@ -193,12 +183,12 @@ class _Request:
 
 class _Env:
     """Driver-side state of one environment: its conjunction draws, the frames that entered its history since the last
-    policy call, whether its policy state must be reset first, its pixel-goal frames and latent plan, its results."""
+    policy call, whether its policy state must be reset first, its latent plan, its results."""
 
     def __init__(self, seed):
         self.rng = random.Random(seed)
         self.history, self.reset = [], False
-        self.goal_rgb = self.goal_depth = self.latent = None
+        self.latent = None
         self.results = []
 
 
@@ -238,7 +228,7 @@ class HabitatVLNEvaluator:
         self.min_depth, self.max_depth = min_depth, max_depth
         self.max_steps_per_episode = max_steps_per_episode
         self.depth_filter, self.vision_cache_frames = depth_filter, vision_cache_frames
-        self.seeds, self.x_init, self.max_new_tokens = seeds, x_init, max_new_tokens
+        self.seeds, self.max_new_tokens = seeds, max_new_tokens
         self.device = torch.device(getattr(model, "device", "cpu"))
         self.reads_depth = mode == "dual_system" and \
             getattr(getattr(model, "config", None), "system1", None) == "navdp_async"
@@ -247,10 +237,10 @@ class HabitatVLNEvaluator:
         self.camera_height = camera_height
         self.intrinsic = intrinsic_matrix(width, height, hfov)
         self.make_follower = _shortest_path_follower if make_follower is None else make_follower
-        self._frames = None
-        if self.device.type == "cuda" and mode == "dual_system":
-            from .preprocess import FramePreprocessor
-            self._frames = FramePreprocessor(self.device, out_size=S1_SIZE)
+        self._frames = self.s1 = None
+        if mode == "dual_system":
+            self._frames = FramePreprocessor(self.device) if self.device.type == "cuda" else None
+            self.s1 = System1Inputs(model, self._frames, x_init)
         self.policy = None
         self.calls = {"s2": 0, "s1": 0, "rounds": 0}
 
@@ -330,33 +320,15 @@ class HabitatVLNEvaluator:
     # ------------------------------------------------------------------ System 1
     def _system1(self, envs, reqs, state):
         """One generate_traj call for the listed environments -> each one's local action chunk (MAX_LOCAL_STEPS ids)."""
-        cur = self._rgb224([r.rgb for r in reqs])
+        cur = self.s1.rgb([r.rgb for r in reqs]).to(torch.bfloat16)
         cur_d = None
         if self.reads_depth:
             cur_d = torch.stack([self.s1_depth(r.depth) for r in reqs]).to(self.device)
-        for k, (e, r) in enumerate(zip(envs, reqs)):
-            if r.goal:
-                state[e].goal_rgb = cur[k].clone()
-                state[e].goal_depth = None if cur_d is None else cur_d[k].clone()
-        rgb = torch.stack([torch.stack((state[e].goal_rgb, cur[k])) for k, e in enumerate(envs)])
-        dep = None
-        if cur_d is not None:
-            dep = torch.stack([torch.stack((state[e].goal_depth, cur_d[k])) for k, e in enumerate(envs)])[..., None]
-        lat = torch.cat([state[e].latent.reshape(1, *state[e].latent.shape[-2:]) for e in envs])
-        kw = {} if self.x_init is None else {"x_init": self.x_init(envs)}
-        with torch.no_grad():
-            traj = self.model.generate_traj(lat, rgb, dep, **kw)
+        traj = self.s1.generate(envs, {e for e, r in zip(envs, reqs) if r.goal}, cur, cur_d,
+                                [state[e].latent for e in envs])
         self.calls["s1"] += 1
         lists = batched_traj_to_actions(traj, len(envs), max_actions=MAX_LOCAL_STEPS)
         return [(list(a) + [STOP] * MAX_LOCAL_STEPS)[:MAX_LOCAL_STEPS] for a in lists]
-
-    def _rgb224(self, frames):
-        """Raw uint8 look-down frames -> bf16 [n, 224, 224, 3] = bf16(Pillow-resized u8) / 255, on the device."""
-        if self._frames is None:
-            u8 = np.stack([np.array(Image.fromarray(np.asarray(f)).convert("RGB").resize((S1_SIZE, S1_SIZE)))
-                           for f in frames])
-            return torch.from_numpy(u8).to(torch.bfloat16) / 255
-        return InternVLAN1AsyncAgent._by_shape(frames, self._frames.rgb).to(torch.bfloat16)
 
     def s1_depth(self, depth):
         """One raw depth observation ([H, W] or [H, W, 1], normalised) -> host bf16 [224, 224]: the reference's filter,
@@ -368,7 +340,7 @@ class HabitatVLNEvaluator:
         d = d * (self.max_depth - self.min_depth) + self.min_depth
         d = d * 1000
         t = torch.as_tensor(np.ascontiguousarray(d.astype(np.uint16) / 1000)).float()
-        t[t > DEPTH_CLIP] = DEPTH_CLIP
+        t[t > SYS1_DEPTH_THRESHOLD] = SYS1_DEPTH_THRESHOLD
         return t.to(torch.bfloat16)
 
     # ------------------------------------------------------------------ one environment (L271-606)
@@ -379,7 +351,8 @@ class HabitatVLNEvaluator:
             obs = env.reset()
             if not env.is_running or obs is None:
                 break
-            st.history, st.reset, st.goal_rgb, st.goal_depth, st.latent = [], True, None, None, None
+            st.history, st.reset, st.latent = [], True, None
+            self.s1.reset([e])
             episode = env.get_current_episode()
             scene_id, episode_id = episode.scene_id.split("/")[-2], int(episode.episode_id)
             instruction = episode.instruction.instruction_text

@@ -23,7 +23,6 @@ name under which the reference evaluator loads that checkpoint in its `system2` 
 """
 from types import SimpleNamespace
 
-import numpy as np
 import torch
 
 from .navdp import NavDP_Policy_DPT_CriticSum_DAT
@@ -310,43 +309,3 @@ class InternVLAN1ForCausalLM:
 
 
 Qwen2_5_VLForConditionalGeneration = InternVLAN1ForCausalLM
-
-
-class S1Output(SimpleNamespace):
-    pass
-
-
-class InternVLAN1Net:
-    """Policy wrapper with the reference's System-1 entry point (internvla_n1_policy.py L200-215)."""
-
-    def __init__(self, model, continuous_traj=True):
-        self.model = model
-        self.continuous_traj = continuous_traj
-
-    def eval(self):
-        return self
-
-    def reset(self):
-        pass
-
-    def s1_step_latent(self, rgb, depth, latent):
-        with torch.no_grad():
-            dp_actions = self.model.generate_traj(traj_latents=latent, images_dp=rgb, depths_dp=depth)
-        B = latent.shape[0]
-        lists = batched_traj_to_actions(dp_actions, B, max_actions=4) if self.continuous_traj else None
-        if lists is None:
-            raise NotImplementedError("chunk_token sampling path: use postprocess.chunk_token on a chosen sample")
-        outs = [S1Output(idx=s1_action_list(a)) for a in lists]
-        return outs[0] if B == 1 else outs
-
-
-def preprocess_s1_inputs(rgb_u8, depth_m, goal_rgb_u8, goal_depth_m, depth_clip=5.0):
-    """S1 input preprocessing of the agent (internvla_n1_agent.py L308-334): uint8 RGB -> [0,1], depth metres clipped,
-    stacked as [goal frame, current frame].  Inputs are already 224x224 numpy arrays (resize happens upstream, PIL)."""
-    def f(x):
-        return np.asarray(x, dtype=np.float32) / 255.0
-    d0 = np.minimum(np.asarray(goal_depth_m, dtype=np.float32), depth_clip)
-    d1 = np.minimum(np.asarray(depth_m, dtype=np.float32), depth_clip)
-    rgbs = torch.from_numpy(np.stack([f(goal_rgb_u8), f(rgb_u8)])).unsqueeze(0)
-    depths = torch.from_numpy(np.stack([d0, d1])).unsqueeze(0).unsqueeze(-1)
-    return rgbs, depths

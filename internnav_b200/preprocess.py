@@ -17,6 +17,9 @@ normalises and cuts it into 14 x 14 x 2 patch rows in numpy.  `QwenImagePreproce
 produces the processor's rows bit for bit (converted to bf16, as the model consumes them): both resizes on
 `n1_resize_rgb_u8` (uint8 output), and rescale + normalise + patchify in one `n1_vl_patchify` launch, since after a
 uint8 resize the processor's arithmetic is a table of the 256 byte values per channel.
+
+`System1Inputs` is the System-1 half of the batched drivers (the real-world agent and the VLN-CE evaluator): the 224 x 224
+RGB frames, each environment's goal frames, the [goal, current] stacks and the `generate_traj` call.
 """
 import math
 import ctypes
@@ -24,11 +27,29 @@ from ctypes import c_void_p
 
 import numpy as np
 import torch
+from PIL import Image
 
 from . import _lib
 from ._lib import VlImage, check
 
+S1_SIZE = 224
 SYS1_DEPTH_THRESHOLD = 5.0
+
+
+def by_shape(frames, fn):
+    """fn over the frames in one call per distinct frame shape (one in all for a fleet of identical cameras).  fn takes a
+    list of frames of one shape and returns one result per frame.  -> the per-frame results in input order: fn's own
+    return value when all frames have one shape, else a list."""
+    groups = {}
+    for k, f in enumerate(frames):
+        groups.setdefault(tuple(np.shape(f)), []).append(k)
+    if len(groups) == 1:
+        return fn(list(frames))
+    out = [None] * len(frames)
+    for idx in groups.values():
+        for k, r in zip(idx, fn([frames[k] for k in idx])):
+            out[k] = r
+    return out
 
 
 def resize_coeffs(in_size, out_size):
@@ -72,7 +93,7 @@ class _ResizePlans:
 
 
 class FramePreprocessor:
-    def __init__(self, device="cuda:0", out_size=224):
+    def __init__(self, device="cuda:0", out_size=S1_SIZE):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("n1b200 has no CPU path: FramePreprocessor needs device='cuda:N'")
@@ -128,6 +149,63 @@ class FramePreprocessor:
         r = self.rgb(torch.from_numpy(rgb)).view(B, 2, self.out, self.out, 3)
         d = self.depth(torch.from_numpy(dep)).view(B, 2, self.out, self.out, 1)
         return r, d
+
+
+class System1Inputs:
+    """System 1 of a batched driver: [goal frame, current frame] of each listed environment -> one `generate_traj` call.
+
+    The current frames are resized to 224 x 224 as the reference's agents resize them with Pillow: on the device by the
+    driver's `FramePreprocessor` (bit-equal), without one by Pillow itself.  The frame of a goal step becomes that
+    environment's goal frame, already resized (the reference resizes the same bytes again on every step, with the same
+    result), until the next goal step or `reset`.  `depth` is the plain resize of the real-world agent; a driver with
+    another depth rule (the VLN-CE evaluator) prepares its depth frames itself.  What happens to the trajectories is the
+    driver's."""
+
+    def __init__(self, model, preprocessor=None, x_init=None):
+        """`preprocessor`: the FramePreprocessor of the driver's CUDA device, or None (Pillow on the host).  `x_init`:
+        None (System 1 draws its initial noise on the device) or a callable env_ids -> noise [len(env_ids) * 32, T, 3]
+        for those environments, in that order."""
+        self.model, self.preprocessor, self.x_init = model, preprocessor, x_init
+        self._goal = {}
+
+    def reset(self, env_ids):
+        for e in env_ids:
+            self._goal.pop(e, None)
+
+    def rgb(self, frames):
+        """Raw uint8 frames [H, W, 3] -> float32 [n, 224, 224, 3] = Pillow-resized / 255, on the driver's device."""
+        if self.preprocessor is None:
+            return torch.from_numpy(np.stack([np.array(Image.fromarray(np.asarray(f)).resize((S1_SIZE, S1_SIZE))) / 255.0
+                                              for f in frames])).float()
+        return self._stack(by_shape(frames, lambda fs: self.preprocessor.rgb(np.stack(fs))))
+
+    def depth(self, frames):
+        """Raw float32 depth [H, W] (or [H, W, 1]) -> float32 [n, 224, 224], Pillow-resized (mode F), no scaling, no
+        clip."""
+        frames = [np.asarray(f, dtype=np.float32).reshape(np.shape(f)[:2]) for f in frames]
+        if self.preprocessor is None:
+            return torch.from_numpy(np.stack([np.array(Image.fromarray(f).resize((S1_SIZE, S1_SIZE))) for f in frames]))
+        resize = lambda fs: self.preprocessor.depth(np.stack(fs), mul=1.0, clip_max=float("inf"))  # noqa: E731
+        return self._stack(by_shape(frames, resize))
+
+    @staticmethod
+    def _stack(rows):
+        return rows if torch.is_tensor(rows) else torch.stack(rows)
+
+    def generate(self, env_ids, goals, rgb, depth, latents):
+        """The listed environments' current frames, prepared by the driver -- rgb [n, 224, 224, 3], depth [n, 224, 224]
+        or None for a System 1 that reads no depth -- and latent plans [.., n_query, H] -> the trajectories of one
+        `generate_traj` call.  The frames of the environments in `goals` become their goal frames first."""
+        for k, e in enumerate(env_ids):
+            if e in goals:
+                self._goal[e] = (rgb[k].clone(), None if depth is None else depth[k].clone())
+        rgb = torch.stack([torch.stack((self._goal[e][0], rgb[k])) for k, e in enumerate(env_ids)])
+        if depth is not None:
+            depth = torch.stack([torch.stack((self._goal[e][1], depth[k])) for k, e in enumerate(env_ids)])[..., None]
+        lat = torch.cat([l.reshape(1, *l.shape[-2:]) for l in latents])
+        kw = {} if self.x_init is None else {"x_init": self.x_init(env_ids)}
+        with torch.no_grad():
+            return self.model.generate_traj(lat, rgb, depth, **kw)
 
 
 def smart_resize(height, width, factor=28, min_pixels=56 * 56, max_pixels=28 * 28 * 1280):
@@ -248,15 +326,9 @@ class QwenImagePreprocessor:
         """images: device uint8 [H, W, 3] frames -> (pixel_values bf16 [N, 1176] on the device, image_grid_thw int64
         [n, 3]), as `processor(images=...)` returns them.  One resize per distinct frame shape, one patchify launch."""
         assert len(images) > 0, "no images"
-        by_shape = {}
-        for i, im in enumerate(images):
+        for im in images:
             assert im.dtype == torch.uint8 and im.ndim == 3 and im.shape[-1] == 3, "images must be uint8 [H, W, 3]"
-            by_shape.setdefault(tuple(im.shape[:2]), []).append(i)
-        resized = [None] * len(images)
-        for (h, w), idx in by_shape.items():
-            out = self.resize(torch.stack([images[i] for i in idx]), self.size(h, w))
-            for k, i in enumerate(idx):
-                resized[i] = out[k]
+        resized = by_shape(images, lambda ims: self.resize(torch.stack(ims), self.size(*ims[0].shape[:2])))
         table = (VlImage * len(images))()
         rows = 0
         for t, r in zip(table, resized):

@@ -12,9 +12,10 @@ def _rel(a, b):
     return ((a - b).norm() / (b.norm() + 1e-12)).item()
 
 
-def test_dual_system_step_matches_oracle_chain():
-    from internnav_b200.internvla_n1 import InternVLAN1ForCausalLM, InternVLAN1Net
+def test_dual_system_step_and_policy_s1_match_oracle_chain():
+    from internnav_b200.internvla_n1 import InternVLAN1ForCausalLM
     from internnav_b200.manifest import random_navdp_state_dict
+    from internnav_b200.policy import InternVLAN1Policy
     from oracle import navdp_oracle as O, qwen_oracle as Q, weights
     torch.backends.cuda.matmul.allow_tf32 = False
     cfg = Q.tiny_cfg()  # hidden 256 -> NavDP vlm_token_dim 256
@@ -73,8 +74,9 @@ def test_dual_system_step_matches_oracle_chain():
     # chained output is the relative one (<= 2x bf16 eager); the per-stage bars are asserted where the stages are tested
     assert e < 4e-2 and e < 2 * e_eager + 2e-3, (e, e_eager)
     # policy wrapper: same trajectories -> same ids as the batched tail
-    pol = InternVLAN1Net(model)
-    outs = pol.s1_step_latent(rgb, dep, mine_lat)
+    pol = InternVLAN1Policy(model, None, num_envs=B)
+    per_env = lambda x: [x[b:b + 1] for b in range(B)]  # noqa: E731
+    outs = pol.s1_step_latent(list(range(B)), per_env(rgb), per_env(dep), per_env(mine_lat))
     assert len(outs) == B and all(isinstance(o.idx, list) for o in outs)
 
 

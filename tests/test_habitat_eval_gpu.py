@@ -25,18 +25,20 @@ def _evaluator(device):
     return HabitatVLNEvaluator(model, H.Processor({}), depth_filter=H.depth_filter)
 
 
-def test_device_s1_rgb_equals_torch_bf16_of_pillow():
-    """One FramePreprocessor call for all frames, cast to bf16 == torch's CPU bf16(Pillow-resized u8) / 255."""
+def test_shared_s1_rgb_cast_to_bf16_equals_torch_bf16_of_pillow():
+    """The evaluator's System-1 RGB: one FramePreprocessor call for all frames (float32 u / 255), cast to bf16 ==
+    torch's CPU bf16(Pillow-resized u8) / 255, and == the Pillow path of an evaluator on the CPU."""
     gpu = _evaluator("cuda:0")
     assert gpu._frames is not None
     frames = [H.observation(5, 0, k)["rgb"] for k in range(6)]
     frames.append(np.resize(np.arange(256, dtype=np.uint8), (480, 640, 3)))   # every byte value
-    got = gpu._rgb224(frames)
-    assert got.is_cuda and got.dtype == torch.bfloat16 and got.shape == (len(frames), 224, 224, 3)
+    f32 = gpu.s1.rgb(frames)
+    assert f32.is_cuda and f32.dtype == torch.float32 and f32.shape == (len(frames), 224, 224, 3)
+    got = f32.to(torch.bfloat16)
     want = torch.stack([torch.tensor(np.array(Image.fromarray(f).resize((224, 224)))).to(torch.bfloat16) / 255
                         for f in frames])
     assert torch.equal(got.cpu().view(torch.int16), want.view(torch.int16))
-    assert torch.equal(got.cpu().view(torch.int16), _evaluator("cpu")._rgb224(frames).view(torch.int16))
+    assert torch.equal(got.cpu().view(torch.int16), _evaluator("cpu").s1.rgb(frames).to(torch.bfloat16).view(torch.int16))
 
 
 @pytest.mark.parametrize("ti", range(len(TRACES)))

@@ -36,17 +36,17 @@ def test_waypoint_kernel_bit_equal_to_numpy(dtype, T, ns):
             assert np.array_equal(got[b], want), (B, b)
 
 
-def test_device_s1_frames_equal_pillow():
+def test_shared_s1_frames_equal_pillow():
     """The agent's device frames (one FramePreprocessor call per step) hold the bytes of the reference's Pillow resize:
     RGB x / 255 exactly as float32, depth in mode F with no scaling or clip."""
     gpu, cpu = R.make_agent(TRACES[:1], "cuda:0")[0], R.make_agent(TRACES[:1], "cpu")[0]
     obs = [R.frame(5, k) for k in range(6)]
-    rgb_gpu = gpu._rgb224([o[0] for o in obs])
+    rgb_gpu = gpu.s1.rgb([o[0] for o in obs])
     assert rgb_gpu.is_cuda and rgb_gpu.dtype == torch.float32
-    assert torch.equal(rgb_gpu.cpu(), cpu._rgb224([o[0] for o in obs]))
+    assert torch.equal(rgb_gpu.cpu(), cpu.s1.rgb([o[0] for o in obs]))
     pil = np.stack([np.array(Image.fromarray(o[0]).resize((224, 224))) / 255 for o in obs])   # the reference, float64
     assert torch.equal(rgb_gpu.cpu(), torch.from_numpy(pil).float())
-    dep_gpu = gpu._depth224([o[1] for o in obs])
+    dep_gpu = gpu.s1.depth([o[1] for o in obs])
     pil_d = np.stack([np.array(Image.fromarray(o[1]).resize((224, 224))) for o in obs])
     assert torch.equal(dep_gpu.cpu(), torch.from_numpy(pil_d)) and float(pil_d.max()) > 5.0   # no clip
 

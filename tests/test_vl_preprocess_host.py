@@ -1,7 +1,8 @@
 """System-2 image preprocessing on the host side (no GPU): the Qwen2-VL arithmetic that QwenImagePreprocessor and
 n1_vl_patchify restate -- smart_resize, the rescale + normalise table, the patch-row order -- against the installed
 transformers processor; which processors qualify for the device path; the argument checks of n1_vl_patchify; the
-text expansion of the policy's device path against the processor's; and a spill-free compile of the kernel."""
+text expansion of the policy's device path against the processor's; the by-shape batching of the resize calls; and a
+spill-free compile of the kernel."""
 import ctypes
 import math
 import os
@@ -17,7 +18,7 @@ from PIL import Image
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from vl_processor import qwen_processor  # noqa: E402
 
-from internnav_b200.preprocess import QwenImagePreprocessor, smart_resize  # noqa: E402
+from internnav_b200.preprocess import QwenImagePreprocessor, by_shape, smart_resize  # noqa: E402
 
 pil_qwen = pytest.importorskip("transformers.models.qwen2_vl.image_processing_pil_qwen2_vl")
 
@@ -163,6 +164,19 @@ def test_expanded_text_ids_match_processor():
         assert torch.equal(mine, ref["input_ids"])
     with pytest.raises(AssertionError, match="placeholders"):
         pol._expand_image_tokens(turns[0][0], grids[:3])
+
+
+def test_by_shape_calls_once_per_shape_and_keeps_input_order():
+    frames = [np.full((2, 3), 0), np.full((4, 5), 1), np.full((2, 3), 2), np.full((4, 5), 3), np.full((1, 1), 4)]
+    calls = []
+
+    def fn(fs):
+        calls.append([int(f.flat[0]) for f in fs])
+        return [10 * int(f.flat[0]) for f in fs]
+    assert by_shape(frames, fn) == [0, 10, 20, 30, 40]
+    assert sorted(calls) == [[0, 2], [1, 3], [4]]
+    batch = torch.arange(6).reshape(3, 2)   # one shape: fn's own result, no regrouping
+    assert by_shape([np.zeros(2)] * 3, lambda fs: batch) is batch
 
 
 def test_patchify_kernel_compiles_without_spills(tmp_path):
