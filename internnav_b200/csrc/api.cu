@@ -88,10 +88,12 @@ inline bf16* B16(void* p) { return static_cast<bf16*>(p); }
 
 // The `expect` feature rows a call writes or reads in pool [pool_rows].  Without a host row table (rows NULL) they are
 // rows 0 .. expect - 1 of a buffer of exactly that many rows.  Otherwise the table has `expect` entries, each a row of
-// the pool, and with `distinct` no row twice (the rows a vision call writes).
+// the pool, and with `distinct` no row twice (the rows a vision call writes).  A call that touches no feature row (a
+// text-only continuation, whose images were all prefilled before) accepts any buffer and an empty table.
 void check_rows(const char* fn, const void* pool, int64_t pool_rows, const int32_t* rows, int64_t n_rows, int64_t expect,
                 bool distinct) {
   const std::string f(fn);
+  if (expect == 0 && n_rows == 0) return;
   if (!rows) {
     if (n_rows != 0 || pool_rows != expect)
       throw Error(N1_ERR_ARG, f + ": without a row table n_rows must be 0 and the features " + std::to_string(expect) +

@@ -98,8 +98,8 @@ class InternVLAN1Policy:
         # whether s2_step computes latent plans (generate_with_latents) or calls generate alone
         self.latent_plans = self.has_system1 and not system2_only
         self.episodes = [_Episode() for _ in range(num_envs)]
-        # K/V cache of each environment's last System-2 conversation, passed back on its look-down turn only (the turn
-        # that continues that conversation; reference internvla_n1_agent_realworld.py L176 / L226 / L239)
+        # K/V cache of each environment's last System-2 conversation, passed back only on a turn that continues that
+        # conversation: here the look-down turn (reference internvla_n1_agent_realworld.py L176 / L226 / L239)
         self._kv_pool = None
         self._kv = [None] * num_envs
         # vision features of images seen in earlier System-2 calls, kept for `vision_cache_frames` resized frames per
@@ -135,23 +135,29 @@ class InternVLAN1Policy:
         n, frame = len(self.episodes), _image_tokens(self.resize_h, self.resize_w)
         return n * self.vision_cache_frames * frame + n * ((self.num_history + 1) * frame + _image_tokens(frame_h, frame_w))
 
-    def _features(self, frame):
+    def _features(self, frame_shape):
         """feature_pool for one call, or None without a vision cache."""
         if self.vision_cache_frames <= 0:
             return None
         if self._feature_pool is None:
-            self._feature_pool = self.model.make_feature_pool(self._feature_rows(*np.asarray(frame).shape[:2]))
+            self._feature_pool = self.model.make_feature_pool(self._feature_rows(*frame_shape))
         return self._feature_pool
 
-    def _caches(self, env_ids, look_downs, frame):
-        """past_key_values for one call, or None when the model keeps no K/V caches."""
+    def _frame_shape(self, rgbs):
+        """(height, width) of the raw frames, which size the pools when they are first made."""
+        return np.asarray(next(r for r in rgbs if r is not None)).shape[:2]
+
+    def _caches(self, env_ids, continues, frame_shape):
+        """past_key_values for one call, or None when the model keeps no K/V caches.  An environment whose turn
+        continues its last conversation (continues[i]) gets that conversation's cache back; every other one starts an
+        empty cache on its own slot."""
         make = getattr(self.model, "make_kv_pool", None)
         if make is None:
             return None
         if self._kv_pool is None:
-            self._kv_pool = make(len(self.episodes), self._kv_capacity(*frame.shape[:2]))
-        return [self._kv[e] if ld and self._kv[e] is not None else self._kv_pool.handle(e)
-                for e, ld in zip(env_ids, look_downs)]
+            self._kv_pool = make(len(self.episodes), self._kv_capacity(*frame_shape))
+        return [self._kv[e] if c and self._kv[e] is not None else self._kv_pool.handle(e)
+                for e, c in zip(env_ids, continues)]
 
     def step_no_infer(self, env_ids, rgbs, depths=None, poses=None):
         if self._vl is not None:
@@ -165,9 +171,12 @@ class InternVLAN1Policy:
 
     def _device_frames(self, rgbs, resize):
         """Raw frames -> device uint8 frames: each uploaded once, those with resize[i] set resized to resize_h x resize_w
-        (Pillow's bicubic), the others kept at full size.  One upload and at most one resize per (shape, resize)."""
+        (Pillow's bicubic), the others kept at full size.  One upload and at most one resize per (shape, resize).  A
+        None entry (a turn that brings no new frame) stays None."""
         groups = {}
         for i, rgb in enumerate(rgbs):
+            if rgb is None:
+                continue
             a = np.asarray(rgb)
             if a.dtype != np.uint8 or a.ndim != 3 or a.shape[-1] != 3:
                 a = np.asarray(Image.fromarray(rgb).convert("RGB"))
@@ -185,8 +194,8 @@ class InternVLAN1Policy:
     # ------------------------------------------------------------------ System 2
     def _build_inputs(self, ep, rgb, instruction, look_down, conjunction=CONJUNCTION):
         """L113-164 for one environment -> processor output (input_ids [1, S], pixel_values, image_grid_thw)."""
-        image = Image.fromarray(rgb).convert("RGB")
-        if not look_down:
+        image = None if rgb is None else Image.fromarray(rgb).convert("RGB")
+        if image is not None and not look_down:
             image = image.resize((self.resize_w, self.resize_h))
         chat = self._chat(ep, image, instruction, look_down, conjunction)
         return self.processor(text=[chat], images=ep.input_images, return_tensors="pt")
@@ -278,9 +287,10 @@ class InternVLAN1Policy:
             prompts = [inp["input_ids"][0].tolist() for _, inp in prepared]
             pixels = torch.cat([inp["pixel_values"] for _, inp in prepared], dim=0)
             grids = torch.cat([torch.stack(list(inp["image_grid_thw"])).reshape(-1, 3) for _, inp in prepared], dim=0)
-        caches = self._caches([env_ids[j] for j, _ in prepared], [look_downs[j] for j, _ in prepared], rgbs[prepared[0][0]])
+        shape = self._frame_shape([rgbs[j] for j, _ in prepared])
+        caches = self._caches([env_ids[j] for j, _ in prepared], [look_downs[j] for j, _ in prepared], shape)
         kw = {} if caches is None else {"past_key_values": caches}
-        features = self._features(rgbs[prepared[0][0]])
+        features = self._features(shape)
         if features is not None:
             kw["feature_pool"] = features
         with torch.no_grad():
@@ -294,18 +304,23 @@ class InternVLAN1Policy:
                 self._kv[env_ids[j]] = out.past_key_values[n]
             ep = self.episodes[env_ids[j]]
             ep.llm_output = self.processor.tokenizer.decode(out.generated[n], skip_special_tokens=True)
-            res = S2Output()
-            try:
-                if re.search(r"\d", ep.llm_output):   # pixel goal "y x" -> [x, y] plus the latent plan (L179-190)
-                    coord = [int(c) for c in re.findall(r"\d+", ep.llm_output)]
-                    res.output_pixel = np.array([int(coord[1]), int(coord[0])])
-                    res.output_latent = out.latents[n:n + 1] if self.latent_plans else None
-                else:
-                    res.output_action = parse_actions(ep.llm_output)
-                results[j] = res
-            except Exception as exc:  # noqa: BLE001 -- e.g. an answer with a single number (IndexError at L181 as well)
-                results[j] = exc
+            results[j] = self._answer(ep, out, n)
         return results
+
+    def _answer(self, ep, out, n):
+        """The S2Output of prompt n of a generate output `out` whose decoded answer is ep.llm_output, or the Exception
+        its parsing raised."""
+        res = S2Output()
+        try:
+            if re.search(r"\d", ep.llm_output):   # pixel goal "y x" -> [x, y] plus the latent plan (L179-190)
+                coord = [int(c) for c in re.findall(r"\d+", ep.llm_output)]
+                res.output_pixel = np.array([int(coord[1]), int(coord[0])])
+                res.output_latent = out.latents[n:n + 1] if self.latent_plans else None
+            else:
+                res.output_action = parse_actions(ep.llm_output)
+            return res
+        except Exception as exc:  # noqa: BLE001 -- e.g. an answer with a single number (IndexError at L181 as well)
+            return exc
 
     # ------------------------------------------------------------------ System 1
     def s1_step_latent(self, env_ids, rgbs, depths, latents):
