@@ -35,7 +35,8 @@ enum {
   N1_ERR_NO_DEVICE = -4,
   N1_ERR_TMA = -5,
   N1_ERR_WEIGHT = -6,
-  N1_ERR_WORKSPACE = -7
+  N1_ERR_WORKSPACE = -7,
+  N1_ERR_KV_PAGES = -8  /* a paged K/V pool has too few free pages for the call; nothing was launched or changed */
 };
 
 enum { N1_F32 = 0, N1_BF16 = 1 };
@@ -167,7 +168,8 @@ int64_t n1_vit_plan_patches(n1_vit_plan p);
  *     pool.  Sequence b then lives in pool slot slots_host[b] (the slots of one batch differ), whose first reused_host[b]
  *     prompt tokens already hold its K/V (0: a fresh sequence).  Positions come from the whole prompt, but only the rows
  *     after that prefix are embedded and prefilled, so the image features cover only the images after it.  The prefix
- *     may not end inside an image, and prompt + max_new_tokens + n_query must fit the pool's capacity. */
+ *     may not end inside an image, and prompt + max_new_tokens + n_query must fit the pool's capacity (a paged pool's
+ *     max_tokens_per_slot).  A plan holds no page numbers: one plan serves any page layout of its pool. */
 int n1_llm_plan_create(n1_handle h, const int32_t* input_ids_host, const int32_t* lens_host, int B,
                        const int32_t* grid_thw_host, int n_img, int max_new_tokens, n1_kv_pool pool,
                        const int32_t* reused_host, const int32_t* slots_host, n1_llm_plan* out, void* stream);
@@ -211,7 +213,11 @@ int n1_llm_prefill(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const 
  * (nullable) = decode passes run.  The call synchronises `stream` (the stop test reads a device counter after every token).
  * On a plan over a K/V pool the call refuses a reused length beyond the rows the slot holds (n1_kv_pool_valid), and
  * afterwards the slot holds the prompt and every generated token whose K/V a pass wrote (all of them when latents_bf16
- * is given, all but the last otherwise). */
+ * is given, all but the last otherwise).
+ * On a paged pool, before anything is launched, every sequence keeps the pages that cover its reused prefix, returns its
+ * other pages and takes pages for prompt + max_new_tokens + n_query rows; when the free pages do not cover that the call
+ * returns N1_ERR_KV_PAGES (the message gives the pages needed and free) and leaves the pool as it was.  Afterwards every
+ * slot of the call returns its pages past ceil(n1_kv_pool_valid / 64). */
 int n1_llm_generate(n1_handle h, n1_llm_plan p, void* ws, size_t ws_bytes, const void* feats_bf16, int64_t feat_rows,
                     const int32_t* image_rows_host, int64_t n_rows, const int32_t* eos_ids_host, int n_eos, int32_t pad_id,
                     int32_t* tokens_host, int32_t* lens_host, void* latents_bf16, int32_t* passes_host, void* stream);
@@ -223,7 +229,16 @@ int n1_kv_pool_create(n1_handle h, int slots, int capacity, n1_kv_pool* out);
 void n1_kv_pool_destroy(n1_kv_pool p);
 size_t n1_kv_pool_bytes(n1_kv_pool p);
 int n1_kv_pool_valid(n1_kv_pool p, int slot); /* rows slot holds, or a negative error code */
-/* copies rows [row, row + n) of a slot in one layer to DEVICE buffers k_out / v_out [n, kv_heads * head_dim] bf16 */
+/* A paged pool: `pages` pages of 64 tokens shared by `slots` conversations of at most max_tokens_per_slot tokens, any
+ * page serving any slot, so memory follows the conversations that are running instead of slots x the longest one.
+ * n1_kv_pool_bytes is pages * 64 tokens.  n1_llm_generate takes and returns pages (see there). */
+int n1_kv_pool_create_paged(n1_handle h, int slots, int pages, int max_tokens_per_slot, n1_kv_pool* out);
+/* ends a slot's conversation: n1_kv_pool_valid becomes 0 and a paged pool gets the slot's pages back */
+int n1_kv_pool_release(n1_kv_pool p, int slot);
+int n1_kv_pool_free_pages(n1_kv_pool p);           /* free pages of a paged pool (0 for a slotted one) */
+int n1_kv_pool_slot_pages(n1_kv_pool p, int slot); /* pages a slot of a paged pool holds (0 for a slotted one) */
+/* copies rows [row, row + n) of a slot in one layer to DEVICE buffers k_out / v_out [n, kv_heads * head_dim] bf16
+ * (a paged pool: through its page table, rows within the pages the slot holds) */
 int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_out, void* v_out, void* stream);
 /* content digest of n_img images, image i = rows [row_off[i], row_off[i + 1]) of bf16 pixels [*, cols] (all DEVICE
  * pointers; cols even) -> digest[i]: equal rows give equal digests, different rows differ with ~2^-64 odds */
@@ -241,6 +256,20 @@ int n1_plan_rows_host(const int32_t* input_ids_host, const int32_t* lens_host, i
                       int n_img, int merge, int vocab, int n_query, int max_new_tokens, int pool_slots, int pool_capacity,
                       const int32_t* reused_host, const int32_t* slots_host, int cap_rows, int32_t* n_rows,
                       int32_t* cu_host, int32_t* kind_host, int32_t* src_host, int32_t* dest_host, int32_t* k_len_host);
+/* the page accounting of a paged K/V pool, without a device: `pages` pages of 64 rows shared by `slots` slots of at
+ * most max_tokens_per_slot rows.  prepare is the step n1_llm_generate takes before it launches: sequence b keeps the
+ * pages covering its first keep_rows[b] rows, returns the rest and takes pages up to need_rows[b] rows (N1_ERR_KV_PAGES
+ * and no change when they do not fit); changed[2] (nullable) = [first, last + 1) slot whose table row changed.  trim
+ * returns a slot's pages past ceil(rows / 64).  table copies the HOST state (each nullable): table [slots,
+ * ceil(max_tokens_per_slot / 64)] (pool page of each slot page, -1 none), held [slots], free list [free pages] (taken
+ * from its end); it returns the free page count. */
+typedef struct n1_kv_pages_s* n1_kv_pages;
+int n1_kv_pages_create(int slots, int max_tokens_per_slot, int pages, n1_kv_pages* out);
+void n1_kv_pages_destroy(n1_kv_pages a);
+int n1_kv_pages_prepare(n1_kv_pages a, int B, const int32_t* slots_host, const int32_t* keep_rows_host,
+                        const int32_t* need_rows_host, int32_t* changed_host);
+int n1_kv_pages_trim(n1_kv_pages a, int slot, int rows);
+int n1_kv_pages_table(n1_kv_pages a, int32_t* table_host, int32_t* held_host, int32_t* free_host);
 /* window_index_host [n_patches/merge^2]; cu_window_host: capacity >= n_patches/merge^2 + 2, count returned in *n_cu */
 int n1_vit_window_index(const int32_t* grid_thw_host, int n_img, int merge, int window, int32_t* window_index_host,
                         int32_t* cu_window_host, int32_t* n_cu, int32_t* pos_hw_host /* [n_patches, 2] or NULL */);
@@ -426,6 +455,12 @@ int n1_op_attention_ex(const void* q, const void* k, const void* v, void* o, int
 int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
                           void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
                           int max_chunk, int heads_q, int heads_kv, float scale, void* stream);
+/* the same over a paged pool: pages (int32, device) is its page table, row0[b] a multiple of 64, and key block n (keys
+ * 64 n .. 64 n + 63) of sequence b lives at rows pages[row0[b] / 64 + n] * 64 .. + 63 of k / v (kv_rows = pages * 64) */
+int n1_op_attention_cache_paged(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv,
+                                int64_t kv_rows, void* o, int ldo, const int32_t* cu_q, const int32_t* ctx,
+                                const int32_t* row0, const int32_t* pages, int batch, int max_chunk, int heads_q,
+                                int heads_kv, float scale, void* stream);
 
 #ifdef __cplusplus
 }

@@ -100,6 +100,15 @@ SYMBOLS = {
     "n1_kv_pool_bytes": (c_size_t, [c_void_p]),
     "n1_kv_pool_valid": (c_int, [c_void_p, c_int]),
     "n1_kv_pool_read": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "n1_kv_pool_create_paged": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "n1_kv_pool_release": (c_int, [c_void_p, c_int]),
+    "n1_kv_pool_free_pages": (c_int, [c_void_p]),
+    "n1_kv_pool_slot_pages": (c_int, [c_void_p, c_int]),
+    "n1_kv_pages_create": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "n1_kv_pages_destroy": (None, [c_void_p]),
+    "n1_kv_pages_prepare": (c_int, [c_void_p, c_int, i32p, i32p, i32p, i32p]),
+    "n1_kv_pages_trim": (c_int, [c_void_p, c_int, c_int]),
+    "n1_kv_pages_table": (c_int, [c_void_p, i32p, i32p, i32p]),
     "n1_image_digest": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
     "n1_rope_index": (c_int, [i32p, c_int, i32p, c_int, c_int, i32p, i32p]),
     "n1_plan_rows_host": (c_int, [i32p, i32p, c_int, i32p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, i32p, i32p,
@@ -170,6 +179,9 @@ SYMBOLS = {
                                 c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
     "n1_op_attention_cache": (c_int, [c_void_p, c_int, ctypes.c_int64, c_void_p, c_void_p, c_int, ctypes.c_int64, c_void_p,
                                       c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "n1_op_attention_cache_paged": (c_int, [c_void_p, c_int, ctypes.c_int64, c_void_p, c_void_p, c_int, ctypes.c_int64,
+                                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                            c_int, c_float, c_void_p]),
 }
 
 OP_RGBD, OP_GOAL, OP_DENOISE = 1, 2, 3
@@ -385,7 +397,25 @@ def attention_test(q, k, v, o, heads_q, heads_kv, head_dim, batch, seq_q=0, seq_
     return ATTN_KERNELS[route[0]], route[1], route[2], route[3]
 
 
-def attention_cache(q, k, v, heads_q, heads_kv, cu_q, ctx, row0, max_chunk, scale=None, out=None):
+def attention_paged_test(q, k, v, o, heads_q, heads_kv, batch, seq_q, k_len, k_row0, pages, k_slot=0, scale=None):
+    """The slotted-cache decode / latent-pass attention (attn_kernel, head_dim 128, causal) over a paged pool: sequence
+    b's keys are its k_len[b] rows of the slotted view starting at k_row0[b] (a multiple of 64; or b * k_slot), whose row
+    r lives at pool row pages[r // 64] * 64 + r % 64 of k / v.  q / o [batch * seq_q, >= heads * 128] views; k_len / k_row0
+    / pages int32 device tensors.  For tests: n1_test_attention_paged is exported but not part of include/n1b200.h."""
+    for t in (q, k, v, o):
+        assert t.dtype == torch.bfloat16 and t.stride(1) == 1
+    assert k.stride(0) == v.stride(0)
+    fn = lib().n1_test_attention_paged
+    fn.restype = c_int
+    fn.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                   c_void_p, c_void_p, ctypes.c_float, c_void_p]
+    vp = lambda t: c_void_p(t.data_ptr())
+    check(fn(vp(q), vp(k), vp(v), vp(o), q.stride(0), k.stride(0), o.stride(0), heads_q, heads_kv, batch, seq_q,
+             ptr(k_len), int(k_slot), ptr(k_row0), ptr(pages), float(128 ** -0.5 if scale is None else scale),
+             stream_ptr()))
+
+
+def attention_cache(q, k, v, heads_q, heads_kv, cu_q, ctx, row0, max_chunk, scale=None, out=None, pages=None):
     """Chunk attention over a slotted K/V cache (head_dim 128): q [rows, >=heads_q*128] packed chunk rows (sequence b at
     cu_q[b] .. cu_q[b + 1]), k / v [kv_rows, heads_kv*128] cache rows (sequence b's keys at row0[b] .. row0[b] + ctx[b] +
     n_b - 1), cu_q / ctx / row0 int32 device tensors -> o [rows, heads_q*128] bf16, bottom-right causal.  `out` may be
@@ -396,10 +426,18 @@ def attention_cache(q, k, v, heads_q, heads_kv, cu_q, ctx, row0, max_chunk, scal
         assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
     o = torch.empty(q.shape[0], heads_q * 128, device=q.device, dtype=torch.bfloat16) if out is None else out
     assert o.dtype == torch.bfloat16 and o.stride(1) == 1 and o.is_cuda
-    check(lib().n1_op_attention_cache(c_void_p(q.data_ptr()), q.stride(0), q.shape[0], c_void_p(k.data_ptr()),
-                                      c_void_p(v.data_ptr()), k.stride(0), k.shape[0], c_void_p(o.data_ptr()), o.stride(0), ptr(cu_q),
-                                      ptr(ctx), ptr(row0), cu_q.numel() - 1, int(max_chunk), heads_q, heads_kv,
-                                      float(128 ** -0.5 if scale is None else scale), stream_ptr()))
+    scale = float(128 ** -0.5 if scale is None else scale)
+    if pages is None:
+        check(lib().n1_op_attention_cache(c_void_p(q.data_ptr()), q.stride(0), q.shape[0], c_void_p(k.data_ptr()),
+                                          c_void_p(v.data_ptr()), k.stride(0), k.shape[0], c_void_p(o.data_ptr()), o.stride(0), ptr(cu_q),
+                                          ptr(ctx), ptr(row0), cu_q.numel() - 1, int(max_chunk), heads_q, heads_kv,
+                                          scale, stream_ptr()))
+        return o
+    assert pages.dtype == torch.int32 and pages.is_cuda and pages.is_contiguous()
+    check(lib().n1_op_attention_cache_paged(c_void_p(q.data_ptr()), q.stride(0), q.shape[0], c_void_p(k.data_ptr()),
+                                            c_void_p(v.data_ptr()), k.stride(0), k.shape[0], c_void_p(o.data_ptr()),
+                                            o.stride(0), ptr(cu_q), ptr(ctx), ptr(row0), ptr(pages), cu_q.numel() - 1,
+                                            int(max_chunk), heads_q, heads_kv, scale, stream_ptr()))
     return o
 
 

@@ -64,12 +64,13 @@ class _Robot:
 
 
 class InternVLAN1AsyncAgent:
-    def __init__(self, args, model=None, processor=None, num_envs=1, x_init=None, vision_cache_frames=0):
+    def __init__(self, args, model=None, processor=None, num_envs=1, x_init=None, vision_cache_frames=0,
+                 kv_pool_tokens=None):
         """args: the reference's (`device`, `model_path`, `resize_w`, `resize_h`, `num_history`, `plan_step_gap`; the gap
         may also be a sequence, one per robot).  Without
         `model` / `processor` the checkpoint at args.model_path is loaded, as the reference does.  `x_init`: None (System 1
         draws its initial noise on the device) or a callable env_ids -> noise [len(env_ids) * 32, T, 3] for those robots,
-        in that order.  `vision_cache_frames`: see InternVLAN1Policy."""
+        in that order.  `vision_cache_frames`, `kv_pool_tokens`: see InternVLAN1Policy."""
         self.device = torch.device(args.device)
         if model is None:
             from .internvla_n1 import InternVLAN1ForCausalLM
@@ -88,7 +89,7 @@ class InternVLAN1AsyncAgent:
         self.plan_step_gap = np.broadcast_to(np.asarray(args.plan_step_gap, dtype=np.int64), (self.num_envs,))
         self.policy = P.InternVLAN1Policy(model, processor, num_envs=num_envs, num_history=args.num_history,
                                           resize_w=args.resize_w, resize_h=args.resize_h, device=self.device,
-                                          vision_cache_frames=vision_cache_frames)
+                                          vision_cache_frames=vision_cache_frames, kv_pool_tokens=kv_pool_tokens)
         self.reads_depth = getattr(getattr(model, "config", None), "system1", None) == "navdp_async"
         self._frames = FramePreprocessor(self.device) if self.device.type == "cuda" else None
         self.s1 = System1Inputs(model, self._frames, x_init)

@@ -1,6 +1,7 @@
 // extern "C" surface of libn1b200.so (include/n1b200.h).  Exceptions stop here and become error codes.
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -31,6 +32,9 @@ struct n1_kv_pool_s {
 };
 struct n1_resize_plan_s {
   ResizePlan* p;
+};
+struct n1_kv_pages_s {
+  PageAlloc a;
 };
 
 namespace {
@@ -381,6 +385,37 @@ void n1_kv_pool_destroy(n1_kv_pool p) {
   delete p->p;
   delete p;
 }
+int n1_kv_pool_create_paged(n1_handle h, int slots, int pages, int max_tokens_per_slot, n1_kv_pool* out) {
+  return guard([&] {
+    use(h);
+    if (!out || slots <= 0 || pages <= 0 || max_tokens_per_slot <= 0)
+      throw Error(N1_ERR_ARG, "n1_kv_pool_create_paged: bad arguments");
+    n1_kv_pool_s* w = new n1_kv_pool_s();
+    try {
+      w->p = h->s2.make_paged_pool(slots, pages, max_tokens_per_slot);
+    } catch (...) {
+      delete w;
+      throw;
+    }
+    *out = w;
+  });
+}
+int n1_kv_pool_release(n1_kv_pool p, int slot) {
+  return guard([&] {
+    if (!p) throw Error(N1_ERR_ARG, "null pool");
+    if (slot < 0 || slot >= p->p->slots) throw Error(N1_ERR_ARG, "n1_kv_pool_release: slot out of range");
+    p->p->valid[slot] = 0;
+    if (p->p->paged()) p->p->pages.trim(slot, 0);
+  });
+}
+int n1_kv_pool_free_pages(n1_kv_pool p) {
+  if (!p) return N1_ERR_ARG;
+  return p->p->paged() ? p->p->pages.free_pages() : 0;
+}
+int n1_kv_pool_slot_pages(n1_kv_pool p, int slot) {
+  if (!p || slot < 0 || slot >= p->p->slots) return N1_ERR_ARG;
+  return p->p->paged() ? p->p->pages.held[slot] : 0;
+}
 size_t n1_kv_pool_bytes(n1_kv_pool p) { return p ? p->p->bytes() : 0; }
 int n1_kv_pool_valid(n1_kv_pool p, int slot) {
   int r = 0;
@@ -397,10 +432,23 @@ int n1_kv_pool_read(n1_kv_pool p, int layer, int slot, int row, int n, void* k_o
     const KvPool& q = *p->p;
     if (layer < 0 || layer >= q.layers || slot < 0 || slot >= q.slots || row < 0 || n < 0 || row + n > q.cap)
       throw Error(N1_ERR_ARG, "n1_kv_pool_read: layer / slot / rows out of range");
-    const long w = q.layer_stride / ((long)q.slots * q.cap);  // kv_heads * head_dim
-    const long off = layer * q.layer_stride + ((long)slot * q.cap + row) * w;
-    N1_CUDA(cudaMemcpyAsync(k_out, q.k + off, (size_t)n * w * sizeof(bf16), cudaMemcpyDeviceToDevice, S(stream)));
-    N1_CUDA(cudaMemcpyAsync(v_out, q.v + off, (size_t)n * w * sizeof(bf16), cudaMemcpyDeviceToDevice, S(stream)));
+    const long w = q.width;
+    if (q.paged() && row + n > q.pages.held[slot] * kPageRows)
+      throw Error(N1_ERR_ARG, "n1_kv_pool_read: rows past the " + std::to_string(q.pages.held[slot]) + " pages slot " +
+                                  std::to_string(slot) + " holds");
+    // contiguous runs: the whole range on a slotted pool, one page at a time on a paged one
+    for (int r = row; r < row + n;) {
+      const int run = q.paged() ? std::min(row + n, (r / kPageRows + 1) * kPageRows) - r : n;
+      const long src = q.paged() ? (long)q.pages.table[(size_t)slot * q.pages.per_slot + r / kPageRows] * kPageRows +
+                                       r % kPageRows
+                                 : (long)slot * q.cap + r;
+      const long off = layer * q.layer_stride + src * w, dst = (long)(r - row) * w;
+      N1_CUDA(cudaMemcpyAsync(B16(k_out) + dst, q.k + off, (size_t)run * w * sizeof(bf16), cudaMemcpyDeviceToDevice,
+                              S(stream)));
+      N1_CUDA(cudaMemcpyAsync(B16(v_out) + dst, q.v + off, (size_t)run * w * sizeof(bf16), cudaMemcpyDeviceToDevice,
+                              S(stream)));
+      r += run;
+    }
   });
 }
 int n1_image_digest(const void* pixels, int64_t cols, const int64_t* row_off, int n_img, uint64_t* digest, void* stream) {
@@ -629,6 +677,43 @@ int n1_plan_rows_host(const int32_t* ids, const int32_t* lens, int B, const int3
     std::copy(r.dest.begin(), r.dest.end(), dest), std::copy(r.len.begin(), r.len.end(), k_len);
   });
 }
+int n1_kv_pages_create(int slots, int max_tokens_per_slot, int pages, n1_kv_pages* out) {
+  return guard([&] {
+    if (!out || max_tokens_per_slot <= 0) throw Error(N1_ERR_ARG, "n1_kv_pages_create: bad arguments");
+    n1_kv_pages_s* w = new n1_kv_pages_s();
+    try {
+      w->a.init(slots, (max_tokens_per_slot + kPageRows - 1) / kPageRows, pages);
+    } catch (...) {
+      delete w;
+      throw;
+    }
+    *out = w;
+  });
+}
+void n1_kv_pages_destroy(n1_kv_pages a) { delete a; }
+int n1_kv_pages_prepare(n1_kv_pages a, int B, const int32_t* slots, const int32_t* keep_rows, const int32_t* need_rows,
+                        int32_t* changed) {
+  return guard([&] {
+    if (!a || B <= 0 || !slots || !keep_rows || !need_rows) throw Error(N1_ERR_ARG, "n1_kv_pages_prepare: bad arguments");
+    const std::pair<int, int> ch = a->a.prepare(B, slots, keep_rows, need_rows);
+    if (changed) changed[0] = ch.first, changed[1] = ch.second;
+  });
+}
+int n1_kv_pages_trim(n1_kv_pages a, int slot, int rows) {
+  return guard([&] {
+    if (!a) throw Error(N1_ERR_ARG, "null page allocator");
+    a->a.trim(slot, rows);
+  });
+}
+int n1_kv_pages_table(n1_kv_pages a, int32_t* table, int32_t* held, int32_t* free_list) {
+  const int e = guard([&] {
+    if (!a) throw Error(N1_ERR_ARG, "null page allocator");
+    if (table) std::copy(a->a.table.begin(), a->a.table.end(), table);
+    if (held) std::copy(a->a.held.begin(), a->a.held.end(), held);
+    if (free_list) std::copy(a->a.free.begin(), a->a.free.end(), free_list);
+  });
+  return e == N1_OK ? a->a.free_pages() : e;
+}
 int n1_rope_index(const int32_t* ids, int len, const int32_t* grid, int n_img, int merge, int32_t* pos3,
                   int32_t* delta) {
   return guard([&] {
@@ -802,13 +887,37 @@ int n1_test_attention(const void* q, const void* k, const void* v, void* o, int 
 int n1_op_attention_cache(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv, int64_t kv_rows,
                           void* o, int ldo, const int32_t* cu_q, const int32_t* ctx, const int32_t* row0, int batch,
                           int max_chunk, int heads_q, int heads_kv, float scale, void* stream) {
+  return n1_op_attention_cache_paged(q, ldq, q_rows, k, v, ldkv, kv_rows, o, ldo, cu_q, ctx, row0, nullptr, batch,
+                                     max_chunk, heads_q, heads_kv, scale, stream);
+}
+int n1_op_attention_cache_paged(const void* q, int ldq, int64_t q_rows, const void* k, const void* v, int ldkv,
+                                int64_t kv_rows, void* o, int ldo, const int32_t* cu_q, const int32_t* ctx,
+                                const int32_t* row0, const int32_t* pages, int batch, int max_chunk, int heads_q,
+                                int heads_kv, float scale, void* stream) {
   return guard([&] {
     if (!q || !k || !v || !o || !cu_q || !ctx || !row0) throw Error(N1_ERR_ARG, "n1_op_attention_cache: null pointer");
     CacheAttnParams a = {};
     a.q = B16(q), a.ldq = ldq, a.q_rows = q_rows, a.k = B16(k), a.v = B16(v), a.ldkv = ldkv, a.kv_rows = kv_rows;
-    a.o = B16(o), a.ldo = ldo, a.cu_q = cu_q, a.ctx = ctx, a.row0 = row0;
+    a.o = B16(o), a.ldo = ldo, a.cu_q = cu_q, a.ctx = ctx, a.row0 = row0, a.pages = pages;
     a.batch = batch, a.max_chunk = max_chunk, a.heads_q = heads_q, a.heads_kv = heads_kv, a.scale = scale;
     attention_cache(a, S(stream));
+  });
+}
+
+// Test entry point, not declared in include/n1b200.h: n1_test_attention's slotted-cache decode / latent-pass attention
+// (k_len, k_slot / k_row0) over a paged pool whose page table is `pages`.
+int n1_test_attention_paged(const void* q, const void* k, const void* v, void* o, int ldq, int ldkv, int ldo, int heads_q,
+                            int heads_kv, int batch, int seq_q, const int32_t* k_len, int k_slot, const int32_t* k_row0,
+                            const int32_t* pages, float scale, void* stream) {
+  return guard([&] {
+    if (!pages || !k_len) throw Error(N1_ERR_ARG, "n1_test_attention_paged: null page table / k_len");
+    AttnParams p = {};
+    p.q = B16(q), p.k = B16(k), p.v = B16(v), p.o = B16(o);
+    p.ldq = ldq, p.ldk = p.ldv = ldkv, p.ldo = ldo;
+    p.heads_q = heads_q, p.heads_kv = heads_kv, p.hd = 128, p.batch = batch, p.seq_q = seq_q;
+    p.kv_div = 1, p.causal = 1, p.scale = scale;
+    p.k_len = k_len, p.k_slot = k_slot, p.k_row0 = k_row0, p.k_pages = pages;
+    attention(p, S(stream));
   });
 }
 

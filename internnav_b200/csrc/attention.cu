@@ -53,7 +53,8 @@ __device__ __forceinline__ void load_tile(uint8_t* sdst, const bf16* gbase, long
   }
 }
 
-template <int HD>
+// PAGED: K/V in a paged pool (p.k_pages); a separate instance, so the contiguous kernels stay exactly as they were
+template <int HD, bool PAGED = false>
 __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
   using C = ACfg<HD>;
   extern __shared__ __align__(16) uint8_t asmem[];
@@ -75,6 +76,11 @@ __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
   const bf16* gq = p.q + (long)q_start * p.ldq + h * HD;
   const bf16* gk = p.k + (long)k_start * p.ldk + hk * HD;
   const bf16* gv = p.v + (long)k_start * p.ldv + hk * HD;
+  // rows from key tile t's contiguous place (k_start + t * 64) to its page of a paged pool
+  auto page_shift = [&](int t) -> long {
+    if constexpr (PAGED) return (long)p.k_pages[(k_start >> 6) + t] * BKV - k_start - t * BKV;
+    return 0;
+  };
 
   const int causal_off = sk - sq;  // key j visible to query i iff j <= i + causal_off
   int kv_end = sk;
@@ -83,8 +89,9 @@ __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
 
   load_tile<HD>(sQ, gq, p.ldq, q0, sq);
   if (ntiles > 0) {
-    load_tile<HD>(sK, gk, p.ldk, 0, sk);
-    load_tile<HD>(sV, gv, p.ldv, 0, sk);
+    const long d = page_shift(0);
+    load_tile<HD>(sK, gk + d * p.ldk, p.ldk, 0, sk);
+    load_tile<HD>(sV, gv + d * p.ldv, p.ldv, 0, sk);
   }
   cp_async_commit();
 
@@ -105,8 +112,9 @@ __global__ void __launch_bounds__(128) attn_kernel(const AttnParams p) {
   for (int t = 0; t < ntiles; ++t) {
     const int st = t & 1;
     if (t + 1 < ntiles) {
-      load_tile<HD>(sK + (st ^ 1) * C::kTileBytes, gk, p.ldk, (t + 1) * BKV, sk);
-      load_tile<HD>(sV + (st ^ 1) * C::kTileBytes, gv, p.ldv, (t + 1) * BKV, sk);
+      const long d = page_shift(t + 1);
+      load_tile<HD>(sK + (st ^ 1) * C::kTileBytes, gk + d * p.ldk, p.ldk, (t + 1) * BKV, sk);
+      load_tile<HD>(sV + (st ^ 1) * C::kTileBytes, gv + d * p.ldv, p.ldv, (t + 1) * BKV, sk);
     }
     cp_async_commit();
     cp_async_wait<1>();
@@ -315,17 +323,17 @@ void launch_attn_small(const AttnParams& p, int G, cudaStream_t stream) {
   N1_CUDA(cudaGetLastError());
 }
 
-template <int HD>
+template <int HD, bool PAGED = false>
 void launch_attn(const AttnParams& p, cudaStream_t stream) {
   using C = ACfg<HD>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
+    cudaFuncSetAttribute(attn_kernel<HD, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
     attr_set = true;
   }
   const int maxq = p.cu_q ? p.max_seq_q : p.seq_q;
   dim3 grid((maxq + BQ - 1) / BQ, p.heads_q, p.batch);
-  attn_kernel<HD><<<grid, 128, C::kSmemBytes, stream>>>(p);
+  attn_kernel<HD, PAGED><<<grid, 128, C::kSmemBytes, stream>>>(p);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }
@@ -365,6 +373,7 @@ void attention(const AttnParams& p, cudaStream_t stream) {
   N1_CHECK(p.ldq % 8 == 0 && p.ldk % 8 == 0 && p.ldv % 8 == 0 && p.ldo % 2 == 0, "attention: misaligned strides");
   N1_CHECK(!p.cu_q || p.max_seq_q > 0, "attention: varlen needs max_seq_q");
   N1_CHECK(p.batch <= 65535 && p.heads_q <= 65535, "attention: grid too large");
+  N1_CHECK(!p.k_pages || (p.k_len && p.hd == 128), "attention: a page table needs k_len and head_dim 128");
   const AttnRoute r = attention_route(p);
   if (r.kernel == ATTN_SHORT) {
     if (r.nkp == 1) launch_attn_small<1>(p, r.group, stream);
@@ -381,7 +390,7 @@ void attention(const AttnParams& p, cudaStream_t stream) {
     case 48: launch_attn<48>(p, stream); break;
     case 64: launch_attn<64>(p, stream); break;
     case 80: launch_attn<80>(p, stream); break;
-    case 128: launch_attn<128>(p, stream); break;
+    case 128: p.k_pages ? launch_attn<128, true>(p, stream) : launch_attn<128>(p, stream); break;
     default: throw Error(-2, "attention: unsupported head_dim " + std::to_string(p.hd));
   }
 }

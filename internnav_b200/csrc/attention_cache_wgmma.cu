@@ -7,7 +7,8 @@
 //
 //   warp 8           producer: Q of the tile (TMA), then K / V in 64-key blocks through a kStages ring (TMA for whole
 //                    blocks; the last, partial block of a sequence is copied by the warp with plain loads and its rows
-//                    past the sequence zeroed, so no row past ctx + n of a slot is ever read)
+//                    past the sequence zeroed, so no row past ctx + n of a slot is ever read).  On a paged pool a
+//                    block is one page: its first row comes from the page table
 //   warpgroups 0-1   S = Q K^T (wgmma m64n64k16) -> online softmax in registers -> O += P V (m64n128k16, P from
 //                    registers, V in place as an MN-major B operand), as attention_wgmma.cu.  O / sum -> global.
 #include <math.h>
@@ -34,7 +35,7 @@ struct CacheArgs {
   int ldkv;
   bf16* o;
   int ldo;
-  const int *cu_q, *ctx, *row0;
+  const int *cu_q, *ctx, *row0, *pages;
   int group, rows_wg;  // G query heads per K/V head, R = 64 / G query rows per warpgroup
   float scale_log2;
 };
@@ -92,12 +93,13 @@ attn_cache_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       uint8_t* sK = sKV + st * kStageBytes;
       uint8_t* sV = sK + kBlockBytes;
       const int key0 = n * BKEY, rem = k_len - key0;
+      const int krow = a.pages ? a.pages[(row0 >> 6) + n] * BKEY : row0 + key0;  // first cache row of the block
       if (rem >= BKEY) {
         if (lane == 0) {
           mbar_arrive_expect_tx(full + st, kStageBytes);
           for (int kb = 0; kb < 2; ++kb) {
-            tma_load_2d(sK + kb * kHalf, &tmK, full + st, kh * HD + kb * 64, row0 + key0);
-            tma_load_2d(sV + kb * kHalf, &tmV, full + st, kh * HD + kb * 64, row0 + key0);
+            tma_load_2d(sK + kb * kHalf, &tmK, full + st, kh * HD + kb * 64, krow);
+            tma_load_2d(sV + kb * kHalf, &tmV, full + st, kh * HD + kb * 64, krow);
           }
         }
       } else {
@@ -106,7 +108,7 @@ attn_cache_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
           const int r = i >> 4, c = i & 15;
           uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
           if (r < rem) {
-            const long g = (long)(row0 + key0 + r) * a.ldkv + kh * HD + c * 8;
+            const long g = (long)(krow + r) * a.ldkv + kh * HD + c * 8;
             kv = *reinterpret_cast<const uint4*>(a.k + g);
             vv = *reinterpret_cast<const uint4*>(a.v + g);
           }
@@ -235,7 +237,7 @@ void attention_cache(const CacheAttnParams& p, cudaStream_t stream) {
   std::call_once(once, [] { cudaFuncSetAttribute(attn_cache_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem); });
   CacheArgs a;
   a.k = p.k, a.v = p.v, a.ldkv = p.ldkv, a.o = p.o, a.ldo = p.ldo;
-  a.cu_q = p.cu_q, a.ctx = p.ctx, a.row0 = p.row0;
+  a.cu_q = p.cu_q, a.ctx = p.ctx, a.row0 = p.row0, a.pages = p.pages;
   a.group = p.heads_q / p.heads_kv;
   a.rows_wg = 64 / a.group;
   a.scale_log2 = p.scale * 1.4426950408889634f;

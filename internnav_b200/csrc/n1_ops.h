@@ -104,6 +104,9 @@ struct AttnParams {
                          //   sequences of <= 320 tokens take the wgmma kernel (attention_wgmma.cu), which needs it for TMA
   const int* k_row0;     // optional with k_len: [batch_kv] first cache row of sequence kb, replacing kb * k_slot (a
                          //   sequence that lives in a slot of a caller-owned K/V pool)
+  const int* k_pages;    // optional with k_len: page table of a paged K/V pool.  The first row of sequence kb (k_row0[kb]
+                         //   or kb * k_slot) is a multiple of 64, and its key tile t lives at cache rows
+                         //   k_pages[first / 64 + t] * 64 .. + 63 instead of first + t * 64 ..
 };
 void attention(const AttnParams& p, cudaStream_t stream);
 // The kernel attention(p) runs: the one routing rule, which attention() dispatches on and n1_test_attention reports.
@@ -124,7 +127,8 @@ void attention_tc128(const AttnParams& p, cudaStream_t stream);
 // Chunk attention over a slotted K/V cache (attention_cache_wgmma.cu), head_dim 128: sequence b has query rows
 // [cu_q[b], cu_q[b + 1]) of q (its tokens ctx[b] .. ctx[b] + n_b - 1) and keys / values at rows row0[b] .. row0[b] +
 // ctx[b] + n_b - 1 of k / v (the cache already holds the chunk's own K/V).  Bottom-right causal mask.  ctx[b] = 0 is a
-// plain prefill.  Rows past ctx[b] + n_b of a slot are never read.
+// plain prefill.  Rows past ctx[b] + n_b of a slot are never read.  With `pages` (a paged K/V pool) row0[b] is a multiple
+// of 64 and key block n of sequence b lives at rows pages[row0[b] / 64 + n] * 64 .. + 63 of k / v.
 struct CacheAttnParams {
   const bf16* q;
   int ldq;
@@ -137,6 +141,7 @@ struct CacheAttnParams {
   const int *cu_q, *ctx, *row0;  // device: [batch + 1], [batch], [batch]
   int batch, max_chunk, heads_q, heads_kv;
   float scale;
+  const int* pages;  // optional, device
 };
 void attention_cache(const CacheAttnParams& p, cudaStream_t stream);
 

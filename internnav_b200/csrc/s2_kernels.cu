@@ -94,15 +94,25 @@ __global__ void build_embeds_kernel(const int* __restrict__ kind, const int* __r
 // after the prompt sit at idx + delta on all three mrope axes, rope2d.py L150-160) and the visible key count.
 __global__ void gen_rows_kernel(const int* __restrict__ len, const int* __restrict__ delta, const int* __restrict__ gen,
                                 int back, int per_seq, int B, int slot, const int* __restrict__ row0,
-                                int* __restrict__ dest_rows, int* __restrict__ pos3, int* __restrict__ k_len) {
+                                const int* __restrict__ pages, int* __restrict__ dest_rows, int* __restrict__ pos3,
+                                int* __restrict__ k_len) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * per_seq) return;
   const int b = i / per_seq, j = i % per_seq;
   const int idx = len[b] + gen[b] - back + j;
-  dest_rows[i] = (row0 ? row0[b] : b * slot) + idx;
+  const int r = (row0 ? row0[b] : b * slot) + idx;
+  dest_rows[i] = pages ? pages[r >> 6] * 64 + (r & 63) : r;
   const int rows = B * per_seq;
   pos3[i] = pos3[rows + i] = pos3[2 * rows + i] = idx + delta[b];
   if (j == per_seq - 1) k_len[b] = idx + 1;
+}
+
+__global__ void page_rows_kernel(const int* __restrict__ rows, const int* __restrict__ pages, int* __restrict__ out,
+                                 long n) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int r = rows[i];
+  out[i] = pages[r >> 6] * 64 + (r & 63);
 }
 
 // K and V column blocks of the packed qkv rows -> rows dest_rows[r] of the layer's cache ([*, kvdim] each)
@@ -227,9 +237,15 @@ void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, con
 }
 
 void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, const int* row0,
-              int* dest_rows, int* pos3, int* k_len, cudaStream_t s) {
-  gen_rows_kernel<<<nblk((long)B * per_seq), 256, 0, s>>>(len, delta, gen, back, per_seq, B, slot, row0, dest_rows, pos3,
-                                                          k_len);
+              const int* pages, int* dest_rows, int* pos3, int* k_len, cudaStream_t s) {
+  gen_rows_kernel<<<nblk((long)B * per_seq), 256, 0, s>>>(len, delta, gen, back, per_seq, B, slot, row0, pages, dest_rows,
+                                                          pos3, k_len);
+  prof_count_launch();
+  N1_CUDA(cudaGetLastError());
+}
+void page_rows(const int* rows, const int* pages, int* out, long n, cudaStream_t s) {
+  if (n <= 0) return;
+  page_rows_kernel<<<nblk(n), 256, 0, s>>>(rows, pages, out, n);
   prof_count_launch();
   N1_CUDA(cudaGetLastError());
 }

@@ -25,10 +25,12 @@ void build_embeds(const int* kind, const int* src, const bf16* embed_tokens, con
 
 // ---- greedy decode with a KV cache (model.generate of internvla_n1_policy.py L169-176, then generate_latents reusing it)
 // Chunk bookkeeping: per sequence the tokens idx = len + gen - back + j (j < per_seq) -> cache rows b * slot + idx
-// (row0[b] + idx when row0 is given: a slot of a K/V pool),
-// mrope positions idx + delta on all three axes ([3, B * per_seq]), k_len[b] = last idx + 1.
+// (row0[b] + idx when row0 is given: a slot of a K/V pool; a row r of that is pool row pages[r / 64] * 64 + r % 64 when
+// the pool is paged), mrope positions idx + delta on all three axes ([3, B * per_seq]), k_len[b] = last idx + 1.
 void gen_rows(const int* len, const int* delta, const int* gen, int back, int per_seq, int B, int slot, const int* row0,
-              int* dest_rows, int* pos3, int* k_len, cudaStream_t s);
+              const int* pages, int* dest_rows, int* pos3, int* k_len, cudaStream_t s);
+// out[i] = pages[rows[i] / 64] * 64 + rows[i] % 64: a plan's K/V rows (slot s at s * cap + position) -> paged pool rows
+void page_rows(const int* rows, const int* pages, int* out, long n, cudaStream_t s);
 // cache_k/v[dest_rows[r], :] = qkv[r, k_off / v_off : + kvdim]
 void kv_append(const bf16* qkv, int ld, int k_off, int v_off, int kvdim, const int* dest_rows, long rows, bf16* cache_k,
                bf16* cache_v, cudaStream_t s);

@@ -230,17 +230,35 @@ VitPlan* S2Model::make_vit_plan(const int32_t* grid, int n_img, cudaStream_t s) 
   return p.release();
 }
 
-KvPool::~KvPool() { cudaFree(k), cudaFree(v); }
+KvPool::~KvPool() { cudaFree(k), cudaFree(v), cudaFree(table); }
 
 KvPool* S2Model::make_pool(int slots, int cap) const {
   N1_CHECK(loaded_, "System-2 weights not loaded");
   N1_CHECK(slots > 0 && cap > 0 && (long)slots * cap < (1L << 31), "kv pool: slots and capacity must be positive");
   std::unique_ptr<KvPool> p(new KvPool());
-  p->slots = slots, p->cap = cap, p->layers = dims.layers;
-  p->layer_stride = (long)slots * cap * dims.kv_heads * dims.head_dim;
+  p->slots = slots, p->cap = cap, p->layers = dims.layers, p->width = dims.kv_heads * dims.head_dim;
+  p->layer_stride = (long)slots * cap * p->width;
   p->valid.assign(slots, 0);
   N1_CUDA(cudaMalloc(&p->k, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
   N1_CUDA(cudaMalloc(&p->v, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
+  return p.release();
+}
+
+KvPool* S2Model::make_paged_pool(int slots, int pages, int max_tokens) const {
+  N1_CHECK(loaded_, "System-2 weights not loaded");
+  N1_CHECK(slots > 0 && pages > 0 && max_tokens > 0, "kv pool: slots, pages and tokens per slot must be positive");
+  const int per_slot = (max_tokens + kPageRows - 1) / kPageRows;
+  N1_CHECK((long)slots * per_slot * kPageRows < (1L << 31), "kv pool: slots x tokens per slot must stay below 2^31");
+  std::unique_ptr<KvPool> p(new KvPool());
+  p->pages.init(slots, per_slot, pages);
+  p->slots = slots, p->cap = per_slot * kPageRows, p->max_tokens = max_tokens;
+  p->layers = dims.layers, p->width = dims.kv_heads * dims.head_dim;
+  p->layer_stride = (long)pages * kPageRows * p->width;
+  p->valid.assign(slots, 0);
+  N1_CUDA(cudaMalloc(&p->k, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
+  N1_CUDA(cudaMalloc(&p->v, (size_t)p->layer_stride * dims.layers * sizeof(bf16)));
+  N1_CUDA(cudaMalloc(&p->table, p->pages.table.size() * sizeof(int)));
+  N1_CUDA(cudaMemcpy(p->table, p->pages.table.data(), p->pages.table.size() * sizeof(int), cudaMemcpyHostToDevice));
   return p.release();
 }
 
@@ -259,7 +277,7 @@ LlmPlan* S2Model::make_llm_plan(const int32_t* ids, const int32_t* lens, int B, 
   PlanArgs a;
   a.merge = dims.v_merge, a.vocab = dims.vocab, a.n_query = dims.n_query, a.max_new = max_new_tokens;
   a.ctx = ctx_in, a.slots = slot_in;
-  if (cont) a.pool_slots = pool->slots, a.pool_cap = pool->cap;
+  if (cont) a.pool_slots = pool->slots, a.pool_cap = pool->cap, a.pool_limit = pool->max_tokens;
   PlanRows r;
   plan_rows(ids, lens, B, grid, n_img, a, r);
   p->B = B, p->n_query = dims.n_query, p->pool = pool;
@@ -393,22 +411,27 @@ size_t S2Model::llm_impl(Carver c, const LlmPlan& p, const bf16* image_feats, bf
   bf16* att = c.take<bf16>(T * H);
   bf16* hid = c.take<bf16>(T * (long)inter_pad_);
   int* image_rows = c.take<int>(p.n_image_tokens);  // last, so the buffers above sit where they sit without a row table
+  const KvPool* paged = kv && p.pool && p.pool->paged() ? p.pool : nullptr;
+  int* dest_paged = paged ? c.take<int>(T) : nullptr;  // the plan's K/V rows mapped through the page table
   if (c.dry()) return c.used();
 
   if (image_rows_host && p.n_image_tokens > 0)
     N1_CUDA(cudaMemcpyAsync(image_rows, image_rows_host, p.n_image_tokens * sizeof(int), cudaMemcpyHostToDevice, s));
   build_embeds(p.kind, p.src, embed_, image_feats, latentq_, x, T, H, s, image_rows_host ? image_rows : nullptr);
+  const int* dest = p.dest_rows;
+  if (paged) page_rows(p.dest_rows, paged->table, dest_paged, T, s), dest = dest_paged;
   for (int l = 0; l < dims.layers; ++l) {
     const Block& b = lblk_[l];
     block_in(b, x, ln, qkv, p.rope, (int)T, H, dims.heads + dims.kv_heads, hd, dims.rms_eps, s);
     if (kv)  // keep the rotated keys and the values of every prompt token for the decode passes
-      kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, dims.kv_heads * hd, p.dest_rows, T,
+      kv_append(qkv, qkv_n, dims.heads * hd, (dims.heads + dims.kv_heads) * hd, dims.kv_heads * hd, dest, T,
                 kv->k + l * kv->layer_stride, kv->v + l * kv->layer_stride, s);
     if (p.any_ctx) {  // continued sequences: the chunk attends to its slot's cached rows (which now include its own)
       CacheAttnParams a = {};
       a.q = qkv, a.ldq = qkv_n, a.q_rows = T;
       a.k = kv->k + l * kv->layer_stride, a.v = kv->v + l * kv->layer_stride, a.ldkv = dims.kv_heads * hd;
-      a.kv_rows = (long)p.pool->slots * p.pool->cap;
+      a.kv_rows = p.pool->rows();
+      a.pages = paged ? paged->table : nullptr;
       a.o = att, a.ldo = H;
       a.cu_q = p.cu, a.ctx = p.ctx, a.row0 = p.row0;
       a.batch = p.B, a.max_chunk = p.max_len, a.heads_q = dims.heads, a.heads_kv = dims.kv_heads;
@@ -464,6 +487,7 @@ AttnParams S2Model::cache_attn(const LlmPlan& p, int per_seq, const int* k_len, 
   a.ldq = (dims.heads + 2 * dims.kv_heads) * hd, a.ldk = a.ldv = dims.kv_heads * hd, a.ldo = dims.hidden;
   a.heads_q = dims.heads, a.heads_kv = dims.kv_heads, a.hd = hd;
   a.batch = p.B, a.seq_q = per_seq, a.k_len = k_len, a.k_slot = p.slot, a.k_row0 = p.row0;
+  a.k_pages = p.pool && p.pool->paged() ? p.pool->table : nullptr;
   a.kv_div = 1, a.causal = 1, a.scale = 1.0f / sqrtf((float)hd);
   return a;
 }
@@ -501,6 +525,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   const int H = dims.hidden, hd = dims.head_dim, B = p.B, nq = dims.n_query;
   const int qkv_n = (dims.heads + 2 * dims.kv_heads) * hd, kvd = dims.kv_heads * hd, half = hd / 2;
   const int R5 = B * (nq + 1);
+  const int* pages = p.pool && p.pool->paged() ? p.pool->table : nullptr;
   KvCache kv;
   if (p.pool) {  // continuation plan: the caller's pool is the cache
     kv.k = p.pool->k, kv.v = p.pool->v, kv.layer_stride = p.pool->layer_stride;
@@ -536,7 +561,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
     N1_CUDA(cudaStreamSynchronize(s));
     if (active == 0) break;
     // 2. one decode pass: the token just sampled is row (len + gen - 1) of its sequence
-    gen_rows(p.d_len, p.d_delta, g.gen, 1, 1, B, p.slot, p.row0, g.dest, g.pos3, g.k_len, s);
+    gen_rows(p.d_len, p.d_delta, g.gen, 1, 1, B, p.slot, p.row0, pages, g.dest, g.pos3, g.k_len, s);
     mrope_table(g.pos3, g.rope, B, half, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
     gather_rows(embed_, g.cur_tok, g.x, B, 1, H, s);
     chunk_pass(g, p, kv, 1, s);
@@ -545,7 +570,7 @@ size_t S2Model::gen_impl(Carver c, const LlmPlan& p, const bf16* image_feats, co
   if (latents) {
     // 3. generate_latents(output_ids, ...) on the cache: the last sampled token has no K/V yet, so the pass covers
     //    [last token, TRAJ x nq]; rows 1..nq of each sequence are the latent plan (internvla_n1.py L327, L345).
-    gen_rows(p.d_len, p.d_delta, g.gen, 1, nq + 1, B, p.slot, p.row0, g.dest, g.pos3, g.k_len, s);
+    gen_rows(p.d_len, p.d_delta, g.gen, 1, nq + 1, B, p.slot, p.row0, pages, g.dest, g.pos3, g.k_len, s);
     mrope_table(g.pos3, g.rope, R5, half, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
     latent_src(g.cur_tok, B, nq, g.kind, g.src, s);
     build_embeds(g.kind, g.src, embed_, nullptr, latentq_, g.x, R5, H, s);
@@ -580,6 +605,17 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
                "llm_generate: sequence " + std::to_string(b) + " reuses " + std::to_string(p.h_ctx[b]) +
                    " rows but slot " + std::to_string(p.h_slot[b]) + " holds " + std::to_string(pool->valid[p.h_slot[b]]));
   if (ws_bytes < ws_generate(p)) throw Error(-7, "llm_generate: workspace too small");
+  if (pool && pool->paged()) {
+    // each sequence keeps the pages of its reused prefix and holds pages for every row the call may write; refused
+    // (N1_ERR_KV_PAGES, nothing launched, the pool unchanged) when the free pages do not cover that
+    std::vector<int32_t> need(p.B);
+    for (int b = 0; b < p.B; ++b) need[b] = p.h_len[b] + p.max_new + p.n_query;
+    const std::pair<int, int> ch = pool->pages.prepare(p.B, p.h_slot.data(), p.h_ctx.data(), need.data());
+    const size_t row = pool->pages.per_slot;
+    if (ch.first < ch.second)
+      N1_CUDA(cudaMemcpyAsync(pool->table + ch.first * row, pool->pages.table.data() + ch.first * row,
+                              (ch.second - ch.first) * row * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
   if (pool)  // rows past ctx are rewritten from here on
     for (int b = 0; b < p.B; ++b) pool->valid[p.h_slot[b]] = p.h_ctx[b];
   p.wait_ready(s);
@@ -588,7 +624,11 @@ void S2Model::llm_generate(const LlmPlan& p, void* ws, size_t ws_bytes, const bf
   // K/V exist for the prompt and every generated token but the last; the latent pass writes the last one too (and the
   // TRAJ rows after it, which are not part of the conversation)
   if (pool)
-    for (int b = 0; b < p.B; ++b) pool->valid[p.h_slot[b]] = p.h_len[b] + out.lens[b] - (latents ? 0 : 1);
+    for (int b = 0; b < p.B; ++b) {
+      const int slot = p.h_slot[b];
+      pool->valid[slot] = p.h_len[b] + out.lens[b] - (latents ? 0 : 1);
+      if (pool->paged()) pool->pages.trim(slot, pool->valid[slot]);  // the TRAJ rows and the unused budget
+    }
 }
 
 }  // namespace n1

@@ -34,13 +34,22 @@ struct VitPlan {
 // Caller-owned K/V cache pool: `slots` conversations of up to `cap` rows each, per decoder layer.  Sized once
 // (n1_kv_pool_create) and never reallocated by a hot call.  valid[s] = rows of slot s whose K/V a pass actually wrote
 // for the conversation's tokens (prompt + generated; never the TRAJ rows of the latent pass).
+// A paged pool (n1_kv_pool_create_paged) holds `pages` pages of 64 rows instead, any of which serves any slot: plans
+// still address slot s at rows s * cap + i (cap = max_pages * 64), and `table` maps such a row to pool row
+// table[row / 64] * 64 + row % 64.  The host PageAlloc is authoritative; llm_generate uploads the rows it changes.
 struct KvPool {
-  bf16 *k = nullptr, *v = nullptr;  // [layers][slots * cap][kv_heads * head_dim]
+  bf16 *k = nullptr, *v = nullptr;  // [layers][rows()][width]
   int slots = 0, cap = 0;
   long layer_stride = 0;
   std::vector<int> valid;
   size_t bytes() const { return 2 * (size_t)layer_stride * layers * sizeof(bf16); }
-  int layers = 0;
+  int layers = 0, width = 0;  // width = kv_heads * head_dim
+  // paged pools only
+  int max_tokens = 0;       // rows one conversation may hold (the plan bound)
+  int* table = nullptr;     // device [slots][cap / 64]
+  PageAlloc pages;
+  bool paged() const { return table != nullptr; }
+  long rows() const { return layer_stride / width; }
   ~KvPool();
 };
 
@@ -98,6 +107,7 @@ class S2Model {
                          int n_img, cudaStream_t s, int max_new_tokens, const int32_t* ctx_host, const int32_t* slot_host,
                          KvPool* pool) const;
   KvPool* make_pool(int slots, int cap) const;
+  KvPool* make_paged_pool(int slots, int pages, int max_tokens_per_slot) const;
 
   size_t ws_vit(const VitPlan& p) const;
   // pixels bf16 [n_patches, 3 * tpatch * patch^2] -> out bf16 [n_patches / merge^2, v_out] (original token order).

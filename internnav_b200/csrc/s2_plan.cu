@@ -138,9 +138,10 @@ void plan_rows(const int32_t* ids, const int32_t* lens, int B, const int32_t* gr
       N1_CHECK(!used[a.slots[b]], "continuation plan: slot " + std::to_string(a.slots[b]) + " used twice in one batch");
       used[a.slots[b]] = 1;
       N1_CHECK(a.ctx[b] >= 0 && a.ctx[b] < lens[b], "continuation plan: reused length must be in [0, prompt length)");
-      N1_CHECK((long)lens[b] + a.max_new + a.n_query <= a.pool_cap,
+      const int limit = a.pool_limit > 0 ? a.pool_limit : a.pool_cap;
+      N1_CHECK((long)lens[b] + a.max_new + a.n_query <= limit,
                "continuation plan: prompt + max_new_tokens + n_query exceeds the pool's slot capacity (" +
-                   std::to_string(a.pool_cap) + ")");
+                   std::to_string(limit) + ")");
       o.ctx.push_back(a.ctx[b]), o.slot_of.push_back(a.slots[b]);
       o.any_ctx |= a.ctx[b] > 0;
     }
@@ -218,6 +219,59 @@ void plan_rows(const int32_t* ids, const int32_t* lens, int B, const int32_t* gr
       for (int i = 0; i < n; ++i) o.dest[o.cu[b] + i] = r0 + c + i;
       if (cont) o.row0.push_back(r0);
     }
+  }
+}
+
+void PageAlloc::init(int s, int ps, int n) {
+  N1_CHECK(s > 0 && ps > 0 && n > 0 && (long)s * ps < (1L << 31) && (long)n * kPageRows < (1L << 31),
+           "kv pages: slots, pages per slot and pages must be positive");
+  slots = s, per_slot = ps, pages = n;
+  table.assign((size_t)s * ps, -1);
+  held.assign(s, 0);
+  free.resize(n);
+  for (int i = 0; i < n; ++i) free[i] = n - 1 - i;  // page 0 on top
+}
+
+std::pair<int, int> PageAlloc::prepare(int B, const int32_t* slot, const int32_t* keep_rows, const int32_t* need_rows) {
+  auto pages_of = [](long rows) { return (int)((rows + kPageRows - 1) / kPageRows); };
+  long give = 0, take = 0;
+  std::vector<char> seen(slots, 0);
+  for (int b = 0; b < B; ++b) {
+    const int s = slot[b];
+    N1_CHECK(s >= 0 && s < slots && !seen[s], "kv pages: slot " + std::to_string(s) + " out of range or used twice");
+    seen[s] = 1;
+    const int keep = pages_of(keep_rows[b]), need = pages_of(need_rows[b]);
+    N1_CHECK(keep_rows[b] >= 0 && keep <= held[s] && keep_rows[b] <= need_rows[b] && need <= per_slot,
+             "kv pages: sequence " + std::to_string(b) + " keeps " + std::to_string(keep_rows[b]) + " of the " +
+                 std::to_string(held[s] * kPageRows) + " rows its slot holds and needs " + std::to_string(need_rows[b]) +
+                 " (at most " + std::to_string(per_slot * kPageRows) + ")");
+    give += held[s] - keep, take += need - keep;
+  }
+  if (take > (long)free.size() + give)
+    throw Error(kErrKvPages, "kv pages: the call needs " + std::to_string(take) + " pages, " +
+                                 std::to_string(free.size() + give) + " are free (" + std::to_string(free.size()) +
+                                 " in the pool, " + std::to_string(give) + " returned by the call's own slots)");
+  for (int b = 0; b < B; ++b) trim(slot[b], keep_rows[b]);
+  int lo = slots, hi = 0;
+  for (int b = 0; b < B; ++b) {
+    const int s = slot[b], need = pages_of(need_rows[b]);
+    if (held[s] >= need) continue;
+    for (int* t = &table[(size_t)s * per_slot]; held[s] < need; ++held[s]) {
+      t[held[s]] = free.back();
+      free.pop_back();
+    }
+    lo = std::min(lo, s), hi = std::max(hi, s + 1);
+  }
+  return lo < hi ? std::make_pair(lo, hi) : std::make_pair(0, 0);
+}
+
+void PageAlloc::trim(int s, int rows) {
+  N1_CHECK(s >= 0 && s < slots && rows >= 0, "kv pages: slot out of range");
+  const int keep = (int)(((long)rows + kPageRows - 1) / kPageRows);
+  int* t = &table[(size_t)s * per_slot];
+  for (; held[s] > keep; --held[s]) {  // last page first, so the slot's first page ends on top of the free list
+    free.push_back(t[held[s] - 1]);
+    t[held[s] - 1] = -1;
   }
 }
 

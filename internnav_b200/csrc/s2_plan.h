@@ -6,6 +6,7 @@
 #pragma once
 #include <stdint.h>
 
+#include <utility>
 #include <vector>
 
 namespace n1 {
@@ -43,6 +44,7 @@ struct PlanArgs {
   const int32_t* ctx = nullptr;
   const int32_t* slots = nullptr;
   int pool_slots = 0, pool_cap = 0;
+  int pool_limit = 0;  // rows one conversation may hold (prompt + max_new + n_query); 0: pool_cap
 };
 struct PlanRows {
   std::vector<int> cu;                  // [B + 1] planned rows per sequence, packed
@@ -58,5 +60,23 @@ struct PlanRows {
 };
 void plan_rows(const int32_t* ids, const int32_t* lens, int B, const int32_t* grid, int n_img, const PlanArgs& a,
                PlanRows& o);
+
+// Page accounting of a paged K/V pool: `pages` pages of kPageRows rows shared by `slots` conversations of at most
+// per_slot pages each.  table[s * per_slot + i] is the pool page that holds rows [i * 64, i * 64 + 64) of slot s (-1: none);
+// a slot always holds pages 0 .. held[s] - 1 of its table row, so a plan's rows (slot s at s * per_slot * 64 + position)
+// map to pool rows through the table alone.  Freed pages go on top of the free list and are taken from there first.
+constexpr int kPageRows = 64;  // = the key block of attn_kernel and attn_cache_kernel: one block is one page
+constexpr int kErrKvPages = -8;  // N1_ERR_KV_PAGES
+struct PageAlloc {
+  int slots = 0, per_slot = 0, pages = 0;
+  std::vector<int> table, held, free;
+  void init(int slots, int per_slot, int pages);
+  // Sequence b (slot slot[b], slots distinct) keeps the pages covering its first keep_rows[b] rows, returns its other
+  // pages and takes pages up to need_rows[b] rows.  Throws Error(kErrKvPages) with the pages needed and free, leaving
+  // every table unchanged, if they do not fit.  -> [lo, hi): the slots whose table rows changed (lo == hi: none).
+  std::pair<int, int> prepare(int B, const int32_t* slot, const int32_t* keep_rows, const int32_t* need_rows);
+  void trim(int slot, int rows);  // return the pages past ceil(rows / 64)
+  int free_pages() const { return (int)free.size(); }
+};
 
 }  // namespace n1

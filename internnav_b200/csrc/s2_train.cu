@@ -127,7 +127,7 @@ void S2Model::train_forward(const LlmPlan& p, void* ws, size_t ws_bytes, const b
   llm_impl(c, p, image_feats, g.ln, s, &t.kv);
   // 2. the n_query TRAJ rows of every sample as one chunk on that cache: rows len .. len + n_query - 1
   N1_CUDA(cudaMemsetAsync(g.gen, 0, p.B * sizeof(int), s));
-  gen_rows(p.d_len, p.d_delta, g.gen, 0, nq, p.B, p.slot, nullptr, g.dest, g.pos3, g.k_len, s);
+  gen_rows(p.d_len, p.d_delta, g.gen, 0, nq, p.B, p.slot, nullptr, nullptr, g.dest, g.pos3, g.k_len, s);
   mrope_table(g.pos3, g.rope, R, hd / 2, dims.mrope[0], dims.mrope[1], dims.rope_theta, s);
   fill_latent_rows_kernel<<<nblk(R), 256, 0, s>>>(g.kind, g.src, R, nq);
   N1_CUDA(cudaGetLastError());

@@ -108,10 +108,10 @@ class DialogPolicy(P.InternVLAN1Policy):
 
     def __init__(self, model, processor, num_envs=1, num_history=8, resize_w=384, resize_h=384, max_new_tokens=128,
                  device=None, vision_cache_frames=0, prompt=PROMPT_DIALOG, append_look_down=False, turn=5,
-                 frame_shape=(480, 640), npc_tokens=128):
+                 frame_shape=(480, 640), npc_tokens=128, kv_pool_tokens=None):
         super().__init__(model, processor, num_envs=num_envs, num_history=num_history, resize_w=resize_w,
                          resize_h=resize_h, max_new_tokens=max_new_tokens, device=device,
-                         vision_cache_frames=vision_cache_frames, system2_only=True)
+                         vision_cache_frames=vision_cache_frames, system2_only=True, kv_pool_tokens=kv_pool_tokens)
         self.episodes = [_DialogEpisode() for _ in range(num_envs)]
         self.prompt, self.append_look_down, self.turn = prompt, append_look_down, int(turn)
         self.frame_shape, self.npc_tokens = tuple(frame_shape), int(npc_tokens)
@@ -228,7 +228,8 @@ class HabitatDialogEvaluator:
     def __init__(self, model, processor, task="instance_dialog", dialog_enabled=False, turn=5, append_look_down=False,
                  num_history=8, resize_w=384, resize_h=384, min_depth=0.0, max_depth=10.0, max_steps_per_episode=500,
                  depth_filter=None, npc=None, make_follower=None, camera_height=None, width=640, height=480, hfov=79,
-                 seeds=None, max_new_tokens=128, vision_cache_frames=0, npc_tokens=128, mode="system2"):
+                 seeds=None, max_new_tokens=128, vision_cache_frames=0, npc_tokens=128, mode="system2",
+                 kv_pool_tokens=None):
         """`task`: the task name ("instance_dialog", "objectnav", "coin", ...); the oracle sentence is in the prompt
         when it contains "dialog" or with `dialog_enabled`.  `turn`: questions the NPC answers per episode.
         `npc([(env_index, env, obs, question), ...]) -> [answer str or None, ...]`: the oracle, called once per round
@@ -265,6 +266,7 @@ class HabitatDialogEvaluator:
         self.intrinsic = intrinsic_matrix(width, height, hfov)
         self.seeds, self.max_new_tokens = seeds, max_new_tokens
         self.vision_cache_frames, self.npc_tokens = vision_cache_frames, npc_tokens
+        self.kv_pool_tokens = kv_pool_tokens  # see InternVLAN1Policy
         self.device = torch.device(getattr(model, "device", "cpu"))
         self.policy = None
         self.calls = {"s2": 0, "npc": 0, "rounds": 0}
@@ -279,7 +281,8 @@ class HabitatDialogEvaluator:
                                        max_new_tokens=self.max_new_tokens, device=self.device,
                                        vision_cache_frames=self.vision_cache_frames, prompt=self.prompt,
                                        append_look_down=self.append_look_down, turn=self.turn,
-                                       frame_shape=self.frame_shape, npc_tokens=self.npc_tokens)
+                                       frame_shape=self.frame_shape, npc_tokens=self.npc_tokens,
+                                       kv_pool_tokens=self.kv_pool_tokens)
         self.policy.reset()
         seeds = list(range(B)) if self.seeds is None else list(self.seeds)
         if len(seeds) != B:

@@ -196,7 +196,7 @@ class HabitatVLNEvaluator:
     def __init__(self, model, processor, num_history=8, resize_w=384, resize_h=384, min_depth=0.0, max_depth=10.0,
                  max_steps_per_episode=500, depth_filter=None, vision_cache_frames=0, seeds=None, x_init=None,
                  max_new_tokens=128, mode="dual_system", camera_height=None, width=640, height=480, hfov=79,
-                 make_follower=None):
+                 make_follower=None, kv_pool_tokens=None):
         """`depth_filter(depth [H, W], blur_type=None)`: the filter the reference applies to every depth frame; needed
         by a System 1 that reads depth and by the system2 mode.  `seeds`: one `random.Random` seed per environment for
         the conjunction draws, as many as `run_*` gets environments (default 0, 1, ...).  `x_init`: None (System 1 draws its noise on the device) or a callable env_ids ->
@@ -228,6 +228,7 @@ class HabitatVLNEvaluator:
         self.min_depth, self.max_depth = min_depth, max_depth
         self.max_steps_per_episode = max_steps_per_episode
         self.depth_filter, self.vision_cache_frames = depth_filter, vision_cache_frames
+        self.kv_pool_tokens = kv_pool_tokens  # see InternVLAN1Policy
         self.seeds, self.max_new_tokens = seeds, max_new_tokens
         self.device = torch.device(getattr(model, "device", "cpu"))
         self.reads_depth = mode == "dual_system" and \
@@ -262,7 +263,7 @@ class HabitatVLNEvaluator:
                                               resize_w=self.resize_w, resize_h=self.resize_h,
                                               max_new_tokens=self.max_new_tokens, device=self.device,
                                               vision_cache_frames=self.vision_cache_frames,
-                                              system2_only=mode == "system2")
+                                              system2_only=mode == "system2", kv_pool_tokens=self.kv_pool_tokens)
         self.policy.reset()
         seeds = list(range(B)) if self.seeds is None else list(self.seeds)
         if len(seeds) != B:

@@ -254,6 +254,12 @@ class InternVLAN1ForCausalLM:
         from .qwen import KVPool
         return KVPool(self._s2, slots, capacity)
 
+    def make_paged_kv_pool(self, slots, tokens, max_tokens_per_slot=None):
+        """A paged K/V cache pool: ceil(tokens / 64) pages of 64 tokens shared by `slots` conversations of up to
+        `max_tokens_per_slot` tokens each (default: the whole pool).  A conversation holds pages for the tokens it has;
+        generate() evicts the least recently used conversations outside a call when the call needs more pages."""
+        return self._s2.make_paged_kv_pool(slots, tokens, max_tokens_per_slot)
+
     def make_feature_pool(self, rows):
         """A vision-feature pool of `rows` merged rows (v_out bf16 each, 7 168 B at the 7B shapes), allocated once; pass it
         as `feature_pool=` to reuse the vision tower's output for images seen in earlier calls."""

@@ -88,7 +88,7 @@ class _Episode:
 
 class InternVLAN1Policy:
     def __init__(self, model, processor, num_envs=1, num_history=8, resize_w=384, resize_h=384, continuous_traj=True,
-                 max_new_tokens=128, device=None, vision_cache_frames=0, system2_only=False):
+                 max_new_tokens=128, device=None, vision_cache_frames=0, system2_only=False, kv_pool_tokens=None):
         self.model, self.processor = model, processor
         self.num_history, self.resize_w, self.resize_h = num_history, resize_w, resize_h
         self.continuous_traj = continuous_traj
@@ -102,6 +102,10 @@ class InternVLAN1Policy:
         # conversation: here the look-down turn (reference internvla_n1_agent_realworld.py L176 / L226 / L239)
         self._kv_pool = None
         self._kv = [None] * num_envs
+        # None: one slot of _kv_capacity tokens per environment.  An integer: a paged pool of that many tokens shared by
+        # all environments (each still bounded by _kv_capacity), which evicts the least recently used conversations
+        # when it runs out of pages
+        self.kv_pool_tokens = None if kv_pool_tokens is None else int(kv_pool_tokens)
         # vision features of images seen in earlier System-2 calls, kept for `vision_cache_frames` resized frames per
         # environment (0: no pool, every call encodes all its images)
         if vision_cache_frames > 0 and getattr(model, "make_feature_pool", None) is None:
@@ -120,6 +124,8 @@ class InternVLAN1Policy:
         for e in (range(len(self.episodes)) if env_ids is None else env_ids):
             self.episodes[e] = _Episode()
             self._kv[e] = None
+            if self._kv_pool is not None and self._kv_pool.paged:
+                self._kv_pool.release(e)
 
     def _kv_capacity(self, frame_h, frame_w):
         """Tokens one environment's slot must hold: a fresh turn (num_history + 1 resized frames), the look-down frame at
@@ -151,11 +157,13 @@ class InternVLAN1Policy:
         """past_key_values for one call, or None when the model keeps no K/V caches.  An environment whose turn
         continues its last conversation (continues[i]) gets that conversation's cache back; every other one starts an
         empty cache on its own slot."""
-        make = getattr(self.model, "make_kv_pool", None)
+        paged = self.kv_pool_tokens is not None
+        make = getattr(self.model, "make_paged_kv_pool" if paged else "make_kv_pool", None)
         if make is None:
             return None
         if self._kv_pool is None:
-            self._kv_pool = make(len(self.episodes), self._kv_capacity(*frame_shape))
+            self._kv_pool = make(len(self.episodes), self.kv_pool_tokens, self._kv_capacity(*frame_shape)) if paged else \
+                make(len(self.episodes), self._kv_capacity(*frame_shape))
         return [self._kv[e] if c and self._kv[e] is not None else self._kv_pool.handle(e)
                 for e, c in zip(env_ids, continues)]
 

@@ -113,23 +113,81 @@ class KVCache:
         return len(self.tokens) if self.version == self.pool.version[self.slot] else 0
 
 
+PAGE_TOKENS = 64  # tokens per page of a paged KVPool
+
+
+def _pages(tokens):
+    return -(-int(tokens) // PAGE_TOKENS)
+
+
 class KVPool:
-    """Caller-owned device memory for `slots` conversations of up to `capacity` tokens, sized once."""
+    """Caller-owned device memory for `slots` conversations of up to `capacity` tokens, sized once.
+
+    With `pages` the pool is paged: `pages` pages of 64 tokens shared by all slots, `capacity` the most one conversation
+    may hold.  A slot holds pages only for the tokens its conversation has, so the pool can be much smaller than slots x
+    capacity; generate() evicts the least recently used conversations when a call needs more pages than are free."""
     _serials = itertools.count()
 
-    def __init__(self, s2, slots, capacity):
+    def __init__(self, s2, slots, capacity, pages=None):
         L = _lib.lib()
         self.s2, self.slots, self.capacity = s2, int(slots), int(capacity)
+        self.pages = None if pages is None else int(pages)
         h = c_void_p()
         with torch.cuda.device(s2.device):
-            check(L.n1_kv_pool_create(s2._h(), self.slots, self.capacity, ctypes.byref(h)))
+            if self.pages is None:
+                check(L.n1_kv_pool_create(s2._h(), self.slots, self.capacity, ctypes.byref(h)))
+            else:
+                check(L.n1_kv_pool_create_paged(s2._h(), self.slots, self.pages, self.capacity, ctypes.byref(h)))
         self._p = h
         self.serial = next(KVPool._serials)  # identifies the pool in System2's plan cache (ids and addresses are reused)
         self.version = [0] * self.slots
+        self.last_use = {}  # slot -> number of the generate() call that last used it (paged pools: eviction order)
+        self.evictions = 0  # conversations generate() released to make room
+
+    @property
+    def paged(self):
+        return self.pages is not None
 
     @property
     def bytes(self):
         return int(_lib.lib().n1_kv_pool_bytes(self._p))
+
+    @property
+    def free_pages(self):
+        return int(_lib.lib().n1_kv_pool_free_pages(self._p))
+
+    def slot_pages(self, slot):
+        r = _lib.lib().n1_kv_pool_slot_pages(self._p, int(slot))
+        if r < 0:
+            check(r)
+        return r
+
+    def release(self, slot):
+        """End the conversation of `slot`: its handles go stale and a paged pool gets its pages back."""
+        check(_lib.lib().n1_kv_pool_release(self._p, int(slot)))
+        self.version[int(slot)] += 1
+        self.last_use.pop(int(slot), None)
+
+    def make_room(self, slots, keep_rows, need_rows):
+        """Pages for one call on a paged pool: sequence b on slots[b] keeps keep_rows[b] rows and needs need_rows[b].
+        Releases the least recently used conversations outside the call until the free pages cover the call.  -> False
+        (nothing released) when even releasing every other conversation would not."""
+        need = sum(_pages(n) - _pages(k) for k, n in zip(keep_rows, need_rows))
+        short = need - self.free_pages - sum(self.slot_pages(s) - _pages(k) for s, k in zip(slots, keep_rows))
+        if short <= 0:
+            return True
+        inside = set(slots)
+        others = sorted((s for s in range(self.slots) if s not in inside and self.slot_pages(s) > 0),
+                        key=lambda s: (self.last_use.get(s, -1), s))
+        if sum(self.slot_pages(s) for s in others) < short:
+            return False
+        for s in others:
+            if short <= 0:
+                break
+            short -= self.slot_pages(s)
+            self.release(s)
+            self.evictions += 1
+        return True
 
     def valid(self, slot):
         r = _lib.lib().n1_kv_pool_valid(self._p, int(slot))
@@ -233,6 +291,13 @@ class System2:
         self._handle = None
         self._vit_plans, self._llm_plans = {}, {}
         self._ws = {}
+        self._calls = 0
+
+    def make_paged_kv_pool(self, slots, tokens, max_tokens_per_slot=None):
+        """A paged KVPool of ceil(tokens / 64) pages for `slots` conversations of at most `max_tokens_per_slot` tokens
+        (default: the whole pool)."""
+        pages = _pages(tokens)
+        return KVPool(self, slots, pages * PAGE_TOKENS if max_tokens_per_slot is None else max_tokens_per_slot, pages)
 
     # ------------------------------------------------------------------ weights
     def load_state_dict(self, state_dict):
@@ -453,7 +518,9 @@ class System2:
         the images after that prefix go through the vision tower and only the rows after it are prefilled.  Afterwards the
         slot holds the new conversation and `self.last_cache` = dict(caches=[one new KVCache per prompt], prefill_rows,
         vit_patches, reused).  A batch in which some conversation does not fit its slot runs as an uncached call and
-        returns None for every cache.
+        returns None for every cache.  On a paged pool the call first takes the pages it needs, releasing the least
+        recently used conversations outside the call (their handles go stale, so their next turn prefills in full); when
+        even that does not make room, the call runs uncached.
         `feature_pool`: an ImageFeaturePool; images it holds skip the vision tower, the others are encoded into it, and
         `self.last_features` = dict(image_hits, vit_patches).  The outputs are byte-identical to a call without it."""
         if image_feats is not None and (feature_pool is not None or past_key_values is not None):
@@ -494,6 +561,9 @@ class System2:
                 keep += [gi + k for k, (st, _, _) in enumerate(imgs) if st >= reused[b]]
                 images.append({st: (n, dg) for st, n, dg in imgs})
                 gi += len(spans)
+            need = [len(p) + int(max_new_tokens) + nq for p in prompts]
+            if pool.paged and not pool.make_room([c.slot for c in caches], reused, need):
+                pool, reused, keep = None, [0] * B, list(range(len(grid_thw)))   # no room even after eviction: uncached
         sizes = [int(t) * int(h) * int(w) for t, h, w in grid_thw]
         feats, table = image_feats, None
         if feature_pool is not None:
@@ -523,6 +593,9 @@ class System2:
                                 len(eos_token_ids), int(pad_token_id), toks, lens, _lib.ptr(lat), ctypes.byref(passes),
                                 _lib.stream_ptr()))
         out = [list(toks[b * max_new_tokens: b * max_new_tokens + lens[b]]) for b in range(B)]
+        self._calls += 1
+        for s_ in slots or ():
+            pool.last_use[s_] = self._calls
         if caches is not None:
             new = [None] * B if pool is None else \
                 [KVCache(pool, s_, (p + o)[:pool.valid(s_)], im) for p, o, s_, im in zip(prompts, out, slots, images)]
